@@ -8,8 +8,8 @@ PPO.update (2 epochs x 2 minibatches of 4096 frames: forward, backward, [all-red
 Adam).  value = world * T * N / t_step  (the reference's perf/fps definition,
 habitat-baselines/habitat_baselines/rl/ppo/ppo_trainer.py:595-598, learner part).
 
-    python bench.py --gpus 1 --steps K --warmup W           # this repo's sm_100a path
-    python bench.py --impl reference ...                     # the UNMODIFIED reference classes (baseline/_ref) on the CPU
+    python bench.py --gpus 1 --steps K --warmup W           # this repo's sm_90a (H100) path
+    python bench.py --impl reference ...                     # the UNMODIFIED reference classes (oracle/_ref) on the CPU
     python bench.py --impl torch_cuda ...                    # ... and on CUDA (TF32 cuDNN, cudnn.benchmark; DDP + NCCL at N > 1)
     torchrun --nproc-per-node N bench.py --gpus N ...        # one rank per GPU, NCCL
 
@@ -100,7 +100,8 @@ def _peaks():
         d = json.load(open(p))
         return dict(hbm=d["hbm_gbs"], bf16=d["bf16_tflops"], bf16_sustained=d.get("bf16_tflops_sustained", d["bf16_tflops"]),
                     src="measured")
-    return dict(hbm=6650.0, bf16=1590.0, bf16_sustained=1400.0, src="fallback")
+    # NVIDIA H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 dense BF16 TFLOP/s -- upper bounds, not measurements
+    return dict(hbm=3350.0, bf16=989.0, bf16_sustained=989.0, src="H100 SXM data sheet")
 
 
 class ClockSampler:
@@ -174,7 +175,7 @@ def _ref_kwargs():
 
 
 def _make_cpu_learner(T=CPU_SAMPLE["T"], N=CPU_SAMPLE["N"]):
-    """The UNMODIFIED reference (baseline/_ref or /root/reference through the import shim): RolloutStorage.compute_returns
+    """The UNMODIFIED reference (oracle/_ref or the reference checkout, through the import shim): RolloutStorage.compute_returns
     + PPO.update on device="cpu" -- the reference's own CPU PPO path."""
     from oracle.ref_learner import ReferenceLearner
 
@@ -307,6 +308,28 @@ def _config(n):
 # ---------------------------------------------------------------------------------------------
 # hb200 arm
 # ---------------------------------------------------------------------------------------------
+_DUMP_PARAM_SAMPLE = 4 << 20   # parameters kept by --dump-outputs (a fixed, seeded sample when the model is larger)
+
+
+def dump_outputs(out_dir, st, policy, metrics):
+    """What the last timed learner step produced, as .npy files in out_dir: its metrics (float64 scalars), the GAE
+    returns it computed (float32 [T+1, N, 1]) and the parameters its optimizer step left (float32, all of them up to
+    _DUMP_PARAM_SAMPLE values, else a sample at indices drawn from a fixed seed).  Inputs are seeded, so two builds run
+    with the same arguments can be compared file by file."""
+    import numpy as np
+
+    os.makedirs(out_dir, exist_ok=True)
+    for k, v in metrics.items():
+        np.save(os.path.join(out_dir, f"metric_{k}.npy"), np.asarray(float(v), dtype=np.float64))
+    np.save(os.path.join(out_dir, "returns.npy"), st.buffers["returns"].detach().float().cpu().numpy())
+    flat = torch.cat([p.detach().float().flatten() for p in policy.parameters()])
+    if flat.numel() > _DUMP_PARAM_SAMPLE:
+        g = torch.Generator().manual_seed(0)
+        idx = torch.randperm(flat.numel(), generator=g)[:_DUMP_PARAM_SAMPLE].sort().values
+        flat = flat[idx.to(flat.device)]
+    np.save(os.path.join(out_dir, "params.npy"), flat.cpu().numpy())
+
+
 def run_hb200(args):
     import habitat_lab_b200 as hb
     from habitat_lab_b200 import ops
@@ -372,6 +395,8 @@ def run_hb200(args):
     ms, metrics = timed(learner_step, args.steps)
     launches = lib.hb200_launch_count() - l0
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, st, policy, metrics)
     frames = world * T * N * args.steps
     value = frames / (ms * 1e-3)
     cross_rank = cross_rank_equality(policy, dev, world) if world > 1 else None
@@ -437,7 +462,7 @@ def run_hb200(args):
             torch_cuda = torch_cuda_measure(dev, world, st.buffers, next_value, args.steps, args.warmup, seed=100)
             torch_cuda["hb200_over_torch_cuda"] = value / torch_cuda["value"]
             torch_cuda["hb200_e2e_over_torch_cuda"] = e2e_value / torch_cuda["value"]
-        except Exception as e:   # e.g. baseline/_ref missing on this box: report, never lose the hb200 line
+        except Exception as e:   # e.g. oracle/_ref not installed: report, never lose the hb200 line
             torch_cuda = {"unavailable": repr(e)[:300]}
     line = None
     if rank == 0:
@@ -643,21 +668,8 @@ def cross_rank_equality(policy, dev, world):
     return out
 
 
-def _ncu_traffic():
-    """DRAM bytes per launch of the most frequent conv kernel, from the committed `ncu --set full` capture of this
-    round (profiles/*_ncu_traffic.json; offline measurement, not taken during the bench run)."""
-    import glob
-    files = sorted(glob.glob(os.path.join(ROOT, "profiles", "*_ncu_traffic.json")))
-    if not files:
-        return None
-    with open(files[-1]) as f:
-        t = json.load(f)
-    return {"kernel": t["kernel"], "dram_bytes_per_launch": t["traffic_bytes_per_launch"],
-            "algorithmic_bytes_per_launch": 2.0 * 2 * 4096 * 32 * 32 * 32, "source": t["source"]}
-
-
 def kernel_roofline(hb, ops, policy, st, dev, peaks):
-    """Live CUDA-event timing of the dominant kernel family (the tcgen05 implicit-GEMM convolutions)
+    """Live CUDA-event timing of the dominant kernel family (the wgmma implicit-GEMM convolutions)
     on the real config-#2 minibatch buffers: algorithmic FLOPs of every conv launch of one
     minibatch pass (forward + dgrad + wgrad) / the summed launch durations."""
     eng = policy._engine_()
@@ -753,11 +765,10 @@ def kernel_roofline(hb, ops, policy, st, dev, peaks):
     flops = sum(v[0] for v in per.values())
     ms = sum(v[1] for v in per.values())
     achieved = flops / (ms * 1e-3) * 1e-12
-    return {"kernel": "conv_halo_ws_kernel / conv_s2_*_kernel / conv_igemm_kernel / conv_*wgrad_kernel (tcgen05, all 21 convs of "
+    return {"kernel": "conv_halo_ws_kernel / conv_s2_*_kernel / conv_igemm_kernel / conv_*wgrad_kernel (wgmma, all 21 convs of "
                       "one 4096-frame minibatch pass, forward + dgrad + wgrad)",
             "bound": "tensor", "achieved": achieved, "peak": peaks["bf16"], "unit": "TFLOP/s",
             "frac": achieved / peaks["bf16"], "peak_source": peaks["src"] + " (burst: kernels timed alone)",
-            "traffic": _ncu_traffic(),
             "speed_of_light": {"note": "per launch max(FLOPs / bf16 peak, (input + output bytes) / HBM peak): the 32- and "
                                        "64-channel layers are HBM-bound, not tensor-bound", "sol_ms": sol[0],
                                "measured_ms": sol[1], "frac": sol[0] / sol[1] if sol[1] else None},
@@ -857,6 +868,8 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-torch-cuda", action="store_true", help="skip the reference PyTorch-CUDA competitor leg")
     ap.add_argument("--sweep", action="store_true", help="BASELINE configs[4]: minibatch-size sweep (1 GPU), one JSON line")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps write what the last one computed (metrics, returns, parameters) as DIR/*.npy")
     args = ap.parse_args()
     select_workload(args.config)
     if args.sweep:

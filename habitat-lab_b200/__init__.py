@@ -1,6 +1,6 @@
-"""hb200 -- B200-native DD-PPO learner hot path behind habitat-baselines' registry API.
+"""hb200 -- H100-native DD-PPO learner hot path behind habitat-baselines' registry API.
 
-The compute path is libhb200.so (hand-written sm_100a CUDA, C ABI in include/hb200.h);
+The compute path is libhb200.so (hand-written sm_90a CUDA, C ABI in include/hb200.h);
 this package is the thin Python host side that mirrors the reference's
 Policy / Updater / Storage interfaces.  There is no CPU or PyTorch fallback.
 """

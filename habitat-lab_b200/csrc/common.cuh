@@ -1,4 +1,4 @@
-// hb200 -- shared device/host helpers for the sm_100a DD-PPO learner kernels.
+// hb200 -- shared device/host helpers for the sm_90a DD-PPO learner kernels.
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
@@ -42,7 +42,19 @@ void set_last_error(const char* fmt, ...);
   } while (0)
 
 static inline int cdiv(long long a, long long b) { return (int)((a + b - 1) / b); }
-constexpr int kNumSMs = 148;  // B200
+
+// ---- deterministic reductions ----------------------------------------------------------------------------------
+// Gradients summed over frames / pixels / K splits are never accumulated with floating-point atomics (their order, and
+// so the result's last bits, would change from run to run).  Kernels write one partial per block into a scratch
+// buffer, and reduce_partials adds them in a fixed order.
+// Per-stream scratch (tgemm.cu): one growing buffer per stream (per graph capture under capture), stream-ordered.
+int stream_workspace(cudaStream_t st, size_t floats, int tiles, float** ws, int** tickets);
+// dst[i] += sum over p = 0 .. nparts-1, in order of fixed chunks, of parts[p * ld + i] for i < count.
+// tmp: min(nparts, kReduceChunks) * count floats of scratch.
+constexpr int kReduceChunks = 32;
+int reduce_partials(const float* parts, int nparts, long long ld, long long count, float* dst, float* tmp,
+                    cudaStream_t st);
+constexpr int kNumSMs = 132;  // H100 SXM
 
 // ---- warp / block reductions ---------------------------------------------------
 __device__ __forceinline__ float warp_sum(float v) {

@@ -1,11 +1,11 @@
-// hb200 -- implicit-GEMM convolution (forward, data gradient, weight gradient) on tcgen05.
+// hb200 -- implicit-GEMM convolution (forward, data gradient, weight gradient) on wgmma.
 //
-// One CTA = one 128-row accumulator tile held in TMEM.  The im2col A tile is gathered from the
-// NHWC bf16 activation tensor straight into shared memory with zero-filling cp.async (padding
-// and stride handled by predication, never materialised), the weight tile is a pre-packed
-// shared-memory image copied verbatim, one elected thread issues tcgen05.mma (kind::f16,
-// bf16 x bf16 -> f32) and the epilogue drains TMEM with tcgen05.ld, fusing the GroupNorm
-// statistics (sum / sum of squares per frame x group) or the residual-gradient add.
+// One CTA = one warpgroup = one 128-row accumulator tile held in registers.  The im2col A tile is gathered from the
+// NHWC activation tensor straight into shared memory with zero-filling cp.async (padding and stride handled by
+// predication, never materialised), the weight tile is a pre-packed shared-memory image copied verbatim, the
+// warpgroup issues wgmma (fp16 x fp16 or bf16 x bf16 -> f32) and the epilogue reads the tile row by row through a
+// shared-memory transpose, fusing the GroupNorm statistics (sum / sum of squares per frame x group) or the
+// residual-gradient add.
 //
 //   forward : D[pixel, co]    = sum_{r,s,ci} X[pixel@(r,s), ci] * W[co, r,s,ci]     (K-major)
 //   dgrad   : D[pixel, ci]    = sum_{r,s,co} dY[pixel@(r,s), co] * W[co, r,s,ci]    (K-major)
@@ -17,16 +17,17 @@
 //             k8 * rows*16 + row*16               (LBO = rows*16, SBO = 128)
 //   layout 1: 128-byte swizzle: (row>>3)*1024 + (row&7)*128 + ((k8 ^ (row&7)) << 4)
 #include "common.cuh"
-#include "umma.cuh"
+#include "wgmma.cuh"
 
 namespace hb200 {
 void count_launch(int n);
 static int g_umma_layout = 1;  // 128-byte swizzle (coalesced gathers); 0 = no-swizzle interleave
 
-using namespace umma;
+using namespace wg;
 
 constexpr int kStages = 3;
 constexpr int kTileM = 128;
+constexpr int kMaxBN = 128;  // N tile: a 128 x 128 fp32 accumulator is 128 registers per thread of the warpgroup
 constexpr int kChunkK = 64;  // bf16 elements per K chunk (8 x 16-byte vectors)
 constexpr int kMaxChunks = 512;  // K = taps * Ci up to 32768 (the 3x3 compression conv of ResNet50 has K = 9 * 1024)
 
@@ -41,6 +42,9 @@ __device__ __forceinline__ uint64_t kmajor_desc(uint32_t base, int kk, int rows_
     return make_smem_desc(base + (uint32_t)(kk * 2 * rows_total * 16), (uint32_t)rows_total * 16, 128, kNoSwizzle);
   return make_smem_desc(base + (uint32_t)(kk * 32), 16, 1024, kSwizzle128B);
 }
+// byte distance from row 0 to row 64 of a K-major operand (8 row groups of SBO bytes)
+template <int LAYOUT>
+constexpr uint32_t kmajor_hi() { return LAYOUT == 0 ? 8 * 128 : 8 * 1024; }
 
 struct ConvArgs {
   const __nv_bfloat16* src;   // gathered activation tensor (x for fwd, dy for dgrad)
@@ -63,15 +67,14 @@ struct ConvArgs {
 template <int BN, int MODE, int LAYOUT, int NST = kStages>
 __global__ void __launch_bounds__(128) conv_igemm_kernel(const ConvArgs a) {
   extern __shared__ __align__(16) uint8_t smem_raw[];
-  __shared__ __align__(8) uint64_t mma_bar[NST];
-  __shared__ uint32_t tmem_slot;
+  __shared__ float stage_buf[kStageFloats];
   constexpr uint32_t kABytes = kTileM * kChunkK * 2;
   constexpr uint32_t kBBytes = BN * kChunkK * 2;
   constexpr uint32_t kStageBytes = kABytes + kBBytes;
-  constexpr uint32_t kTmemCols = BN < 32 ? 32 : BN;
+  static_assert(BN <= kMaxBN, "conv: N tile");
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
 
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int tid = threadIdx.x, lane = tid & 31;
   const int n0 = blockIdx.y * BN;
   __shared__ short chunk_ids[kMaxChunks];
   __shared__ int n_valid_s;
@@ -124,16 +127,7 @@ __global__ void __launch_bounds__(128) conv_igemm_kernel(const ConvArgs a) {
     n_valid_s = nv;
   }
 
-  if (tid == 0) {
-#pragma unroll
-    for (int s = 0; s < NST; ++s) mbar_init(&mma_bar[s], 1);
-    mbar_fence_init();
-  }
-  if (warp == 0) tmem_alloc(&tmem_slot, kTmemCols);
-  fence_before_sync();
   __syncthreads();
-  fence_after_sync();
-  const uint32_t tmem_base = tmem_slot;
   const int n_valid = n_valid_s;
   const int taps = a.kh * a.kw;
   // the image is [packed tile][chunk][wbn rows x 64]; in the 128B-swizzle layout a BN-row slice of a packed tile is a
@@ -145,7 +139,7 @@ __global__ void __launch_bounds__(128) conv_igemm_kernel(const ConvArgs a) {
   // LAYOUT 1: the 8 rows this thread gathers for (row = tid/8 + 16 i) never change -> their pixel origin lives in
   // registers (frame base, first input row / column of the window; an out-of-range row gets an origin no tap can reach).
   // Per chunk and row that leaves two adds, two unsigned range checks and the address (this loop was 440 warp
-  // instructions per chunk and the whole cost of the few-CTA launches: ncu, one warp per scheduler, 9 % issue).
+  // instructions per chunk and the whole cost of the few-CTA launches, where one warp per scheduler hides nothing).
   int rbase[8], rh[8], rw[8];
   uint32_t soff[8];
   const int jv = tid & 7;
@@ -234,7 +228,8 @@ __global__ void __launch_bounds__(128) conv_igemm_kernel(const ConvArgs a) {
   };
 
   // forward: fp16 activations x fp16 weight image; dgrad: bf16 gradients x bf16 transposed weight image
-  constexpr uint32_t idesc = MODE == 0 ? make_idesc_f16(kTileM, BN, 0, 0, kFmtF16, kFmtF16) : make_idesc_bf16(kTileM, BN, 0, 0);
+  constexpr int kT = MODE == 0 ? kF16 : kBF16;
+  float acc_t[BN];
   // ---- software pipeline: cp.async runs NST-1 chunks ahead of the tensor core ----
 #pragma unroll
   for (int c = 0; c < NST - 1; ++c) {
@@ -246,43 +241,35 @@ __global__ void __launch_bounds__(128) conv_igemm_kernel(const ConvArgs a) {
     cp_async_wait<NST - 2>();
     fence_proxy_async_smem();
     __syncthreads();
-    if (tid == 0) {
-      fence_after_sync();
+    {
       const uint32_t sa = smem_base + stage * kStageBytes;
       const uint32_t sb = sa + kABytes;
+      wgmma_fence();
 #pragma unroll
       for (int kk = 0; kk < kChunkK / 16; ++kk)
-        mma_bf16_ss(tmem_base, kmajor_desc<LAYOUT>(sa, kk, kTileM), kmajor_desc<LAYOUT>(sb, kk, BN),
-                    idesc, (c > 0 || kk > 0) ? 1u : 0u);
-      mma_commit(&mma_bar[stage]);
+        mma128<BN, kT>(acc_t, kmajor_desc<LAYOUT>(sa, kk, kTileM), kmajor_hi<LAYOUT>(), kmajor_desc<LAYOUT>(sb, kk, BN),
+                       (c > 0 || kk > 0) ? 1u : 0u);
+      wgmma_commit();
     }
     const int nc = c + NST - 1;
     if (nc < n_valid) {
-      if (c >= 1) mbar_wait(&mma_bar[(c - 1) % NST], ((c - 1) / NST) & 1);
+      wgmma_wait<1>();   // the MMAs of chunk c-1 have read stage nc % NST
       load_chunk(chunk_ids[nc], nc % NST);
     }
     cp_async_commit();
   }
-  if (n_valid > 0) {
-    const int last = n_valid - 1;
-    mbar_wait(&mma_bar[last % NST], (last / NST) & 1);
-  }
-  fence_after_sync();
+  wgmma_wait<0>();
+  acc_fence(acc_t);
 
-  // ---- epilogue: TMEM -> registers -> (stats | + addend) -> bf16 NHWC ----
-  const uint32_t taddr = tmem_base + ((uint32_t)(warp * 32) << 16);
+  // ---- epilogue: registers -> (stats | + addend) -> fp16 / bf16 NHWC ----
   const int hw = a.OH * a.OW;
   int seg = 1;  // lanes of a warp that share a frame (power of two), else 1
   if ((hw & (hw - 1)) == 0) seg = hw < 32 ? hw : 32;
-#pragma unroll 1
+#pragma unroll
   for (int col0 = 0; col0 < BN; col0 += 32) {
     float acc[32];
     if (n_valid > 0) {
-      uint32_t r[32];
-      tmem_ld32(taddr + col0, r);
-      tmem_ld_wait();
-#pragma unroll
-      for (int j = 0; j < 32; ++j) acc[j] = __uint_as_float(r[j]);
+      acc_row32(acc_t, col0, stage_buf, acc);
     } else {
 #pragma unroll
       for (int j = 0; j < 32; ++j) acc[j] = 0.f;
@@ -372,9 +359,6 @@ __global__ void __launch_bounds__(128) conv_igemm_kernel(const ConvArgs a) {
       }
     }
   }
-  fence_before_sync();
-  __syncthreads();
-  if (warp == 0) tmem_dealloc(tmem_base, kTmemCols);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -383,7 +367,7 @@ __global__ void __launch_bounds__(128) conv_igemm_kernel(const ConvArgs a) {
 struct WgradArgs {
   const __nv_bfloat16* x;
   const __nv_bfloat16* dy;
-  float* dw;  // [(tap, ci)][Co]
+  float* dw;  // partials [split = blockIdx.z][(tap, ci)][Co], summed in split order by reduce_partials
   int B, Hi, Wi, Ci, Ho, Wo, Co, kh, kw, stride, pad;
   int P;       // output pixels B*Ho*Wo
   int KW;      // taps * Ci (valid rows)
@@ -394,16 +378,15 @@ struct WgradArgs {
 template <int BN>
 __global__ void __launch_bounds__(128) conv_wgrad_kernel(const WgradArgs a) {
   extern __shared__ __align__(16) uint8_t smem_raw[];
-  __shared__ __align__(8) uint64_t mma_bar[kStages];
-  __shared__ uint32_t tmem_slot;
+  __shared__ float stage_buf[kStageFloats];
   constexpr uint32_t kABytes = kTileM * kChunkK * 2;
   constexpr uint32_t kBBytes = BN * kChunkK * 2;
   constexpr uint32_t kStageBytes = kABytes + kBBytes;
-  constexpr uint32_t kTmemCols = BN < 32 ? 32 : BN;
   constexpr uint32_t kLboA = (kTileM / 8) * 128, kLboB = (BN / 8) * 128;
+  static_assert(BN <= kMaxBN, "conv_wgrad: N tile");
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
 
-  const int tid = threadIdx.x, warp = tid >> 5;
+  const int tid = threadIdx.x;
   const int row_base = blockIdx.x * kTileM;
   const int n0 = blockIdx.y * BN;
   const long long total_chunks = ((long long)a.P + kChunkK - 1) / kChunkK;
@@ -412,17 +395,6 @@ __global__ void __launch_bounds__(128) conv_wgrad_kernel(const WgradArgs a) {
   if (c_end > total_chunks) c_end = total_chunks;
   const int nchunks = (int)(c_end - c_begin);
   if (nchunks <= 0) return;
-
-  if (tid == 0) {
-#pragma unroll
-    for (int s = 0; s < kStages; ++s) mbar_init(&mma_bar[s], 1);
-    mbar_fence_init();
-  }
-  if (warp == 0) tmem_alloc(&tmem_slot, kTmemCols);
-  fence_before_sync();
-  __syncthreads();
-  fence_after_sync();
-  const uint32_t tmem_base = tmem_slot;
 
   const int kpix = tid & 63;    // pixel within the chunk handled by this thread
   const int half = tid >> 6;    // 0/1
@@ -464,9 +436,9 @@ __global__ void __launch_bounds__(128) conv_wgrad_kernel(const WgradArgs a) {
     }
   };
 
-  // A = the bf16 twin of the forward activations, B = output gradients dy (bf16).  tcgen05 kind::f16 rejects mixed
-  // fp16 x bf16 operands (illegal-instruction fault on B200), so the forward kernels write a bf16-rounded copy of x
-  constexpr uint32_t idesc = make_idesc_bf16(kTileM, BN, 1, 1);
+  // A = the bf16 twin of the forward activations, B = output gradients dy (bf16).  The tensor core has no mixed
+  // fp16 x bf16 form, so the forward kernels write a bf16-rounded copy of x
+  float acc_t[BN];
 #pragma unroll
   for (int c = 0; c < kStages - 1; ++c) {
     if (c < nchunks) load_chunk(c, c);
@@ -477,75 +449,56 @@ __global__ void __launch_bounds__(128) conv_wgrad_kernel(const WgradArgs a) {
     cp_async_wait<kStages - 2>();
     fence_proxy_async_smem();
     __syncthreads();
-    if (tid == 0) {
-      fence_after_sync();
+    {
       const uint32_t sa = smem_base + stage * kStageBytes;
       const uint32_t sb = sa + kABytes;
+      wgmma_fence();
 #pragma unroll
       for (int kk = 0; kk < kChunkK / 16; ++kk) {
         // MN-major, no swizzle: SBO = stride between 8-element MN blocks, LBO = between 8-k blocks
         const uint64_t da = make_smem_desc(sa + kk * 2 * kLboA, kLboA, 128, kNoSwizzle);
         const uint64_t db = make_smem_desc(sb + kk * 2 * kLboB, kLboB, 128, kNoSwizzle);
-        mma_bf16_ss(tmem_base, da, db, idesc, (c > 0 || kk > 0) ? 1u : 0u);
+        mma128<BN, kBF16, 1, 1>(acc_t, da, 8 * 128, db, (c > 0 || kk > 0) ? 1u : 0u);
       }
-      mma_commit(&mma_bar[stage]);
+      wgmma_commit();
     }
     const int nc = c + kStages - 1;
     if (nc < nchunks) {
-      if (c >= 1) mbar_wait(&mma_bar[(c - 1) % kStages], ((c - 1) / kStages) & 1);
+      wgmma_wait<1>();   // the MMAs of chunk c-1 have read stage nc % kStages
       load_chunk(nc, nc % kStages);
     }
     cp_async_commit();
   }
-  {
-    const int last = nchunks - 1;
-    mbar_wait(&mma_bar[last % kStages], (last / kStages) & 1);
-  }
-  fence_after_sync();
+  wgmma_wait<0>();
+  acc_fence(acc_t);
 
-  const uint32_t taddr = tmem_base + ((uint32_t)(warp * 32) << 16);
   const int row = row_base + tid;
-#pragma unroll 1
-  for (int col0 = 0; col0 < BN; col0 += 32) {
-    uint32_t r[32];
-    tmem_ld32(taddr + col0, r);
-    tmem_ld_wait();
-    if (row < a.KW) {
-      float* dst = a.dw + (size_t)row * a.Co + n0 + col0;
 #pragma unroll
-      for (int j = 0; j < 32; j += 4)
-        red_add_v4(dst + j, __uint_as_float(r[j]), __uint_as_float(r[j + 1]), __uint_as_float(r[j + 2]),
-                   __uint_as_float(r[j + 3]));
+  for (int col0 = 0; col0 < BN; col0 += 32) {
+    float r[32];
+    acc_row32(acc_t, col0, stage_buf, r);
+    if (row < a.KW) {
+      float* dst = a.dw + ((size_t)blockIdx.z * a.KW + row) * a.Co + n0 + col0;
+#pragma unroll
+      for (int j = 0; j < 32; j += 4) *reinterpret_cast<float4*>(dst + j) = make_float4(r[j], r[j + 1], r[j + 2], r[j + 3]);
     }
   }
-  fence_before_sync();
-  __syncthreads();
-  if (warp == 0) tmem_dealloc(tmem_base, kTmemCols);
 }
 
 // ------------------------------------------------------------------------------------------
 // minimal synchronous GEMM used to pin the descriptor encodings on hardware
 // ------------------------------------------------------------------------------------------
-template <int LAYOUT, int MNMAJOR>
+template <int LAYOUT, int MNMAJOR, int N, int T>
 __global__ void __launch_bounds__(128)
 umma_probe_kernel(const __nv_bfloat16* __restrict__ A, const __nv_bfloat16* __restrict__ Bm,
-                  float* __restrict__ D, int M, int N, int K, int a_fmt, int b_fmt) {
+                  float* __restrict__ D, int M, int K) {
   extern __shared__ __align__(16) uint8_t smem_raw[];
-  __shared__ __align__(8) uint64_t bar;
-  __shared__ uint32_t tmem_slot;
+  __shared__ float stage_buf[kStageFloats];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t sa = smem_base, sb = smem_base + kTileM * kChunkK * 2;
-  const int tid = threadIdx.x, warp = tid >> 5;
+  const int tid = threadIdx.x;
   const int m0 = blockIdx.x * kTileM;
-  uint32_t ncols = 32;
-  while ((int)ncols < N) ncols <<= 1;
-  if (tid == 0) { mbar_init(&bar, 1); mbar_fence_init(); }
-  if (warp == 0) tmem_alloc(&tmem_slot, ncols);
-  fence_before_sync();
-  __syncthreads();
-  fence_after_sync();
-  const uint32_t tmem_base = tmem_slot;
-  const uint32_t idesc = make_idesc_f16(kTileM, N, MNMAJOR, MNMAJOR, a_fmt, b_fmt);
+  float acc_t[N];
   const int nchunks = K / kChunkK;
   for (int c = 0; c < nchunks; ++c) {
     if (!MNMAJOR) {
@@ -580,36 +533,49 @@ umma_probe_kernel(const __nv_bfloat16* __restrict__ A, const __nv_bfloat16* __re
     }
     fence_proxy_async_smem();
     __syncthreads();
-    if (tid == 0) {
-      fence_after_sync();
-      for (int kk = 0; kk < kChunkK / 16; ++kk) {
-        uint64_t da, db;
-        if (!MNMAJOR) {
-          da = kmajor_desc<LAYOUT>(sa, kk, kTileM);
-          db = kmajor_desc<LAYOUT>(sb, kk, N);
-        } else {
-          const uint32_t lboA = (kTileM / 8) * 128, lboB = (uint32_t)(N / 8) * 128;
-          da = make_smem_desc(sa + kk * 2 * lboA, lboA, 128, kNoSwizzle);
-          db = make_smem_desc(sb + kk * 2 * lboB, lboB, 128, kNoSwizzle);
-        }
-        mma_bf16_ss(tmem_base, da, db, idesc, (c > 0 || kk > 0) ? 1u : 0u);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < kChunkK / 16; ++kk) {
+      uint64_t da, db;
+      uint32_t a_hi;
+      if (!MNMAJOR) {
+        da = kmajor_desc<LAYOUT>(sa, kk, kTileM);
+        db = kmajor_desc<LAYOUT>(sb, kk, N);
+        a_hi = kmajor_hi<LAYOUT>();
+      } else {
+        const uint32_t lboA = (kTileM / 8) * 128, lboB = (uint32_t)(N / 8) * 128;
+        da = make_smem_desc(sa + kk * 2 * lboA, lboA, 128, kNoSwizzle);
+        db = make_smem_desc(sb + kk * 2 * lboB, lboB, 128, kNoSwizzle);
+        a_hi = 8 * 128;
       }
-      mma_commit(&bar);
+      mma128<N, T, MNMAJOR, MNMAJOR>(acc_t, da, a_hi, db, (c > 0 || kk > 0) ? 1u : 0u);
     }
-    mbar_wait(&bar, c & 1);  // fully synchronous: smem is reused next iteration
-    fence_after_sync();
+    wgmma_commit();
+    wgmma_wait<0>();  // fully synchronous: smem is reused next iteration
     __syncthreads();
   }
-  const uint32_t taddr = tmem_base + ((uint32_t)(warp * 32) << 16);
-  for (int col0 = 0; col0 < N; col0 += 16) {
-    uint32_t r[16];
-    tmem_ld16(taddr + col0, r);
-    tmem_ld_wait();
-    for (int j = 0; j < 16; ++j) D[(size_t)(m0 + tid) * N + col0 + j] = __uint_as_float(r[j]);
+  acc_fence(acc_t);
+  if (N >= 32) {
+#pragma unroll
+    for (int col0 = 0; col0 < N; col0 += 32) {
+      float r[32];
+      acc_row32(acc_t, col0, stage_buf, r);
+      for (int j = 0; j < 32; ++j) D[(size_t)(m0 + tid) * N + col0 + j] = r[j];
+    }
+  } else {   // N = 16: straight from the fragment
+    const int w = tid >> 5, l = tid & 31;
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+      for (int i = 0; i < N / 8; ++i) {
+        const int row = m0 + h * 64 + 16 * w + (l >> 2), col = 8 * i + 2 * (l & 3);
+        const float* f = &acc_t[h * (N / 2) + 4 * i];
+        D[(size_t)row * N + col] = f[0];
+        D[(size_t)row * N + col + 1] = f[1];
+        D[(size_t)(row + 8) * N + col] = f[2];
+        D[(size_t)(row + 8) * N + col + 1] = f[3];
+      }
   }
-  fence_before_sync();
-  __syncthreads();
-  if (warp == 0) tmem_dealloc(tmem_base, ncols);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -681,13 +647,13 @@ static int ilog2(int v) {
   return l;
 }
 static bool is_pow2(int v) { return v > 0 && (v & (v - 1)) == 0; }
-static int pick_bn(int n) { return n >= 256 ? 256 : n; }
+static int pick_bn(int n) { return n >= kMaxBN ? kMaxBN : n; }
 
 template <int MODE>
 static int launch_igemm(ConvArgs a, int BN, cudaStream_t st) {
   a.wbn = BN;
-  // few output rows (the actor's 64-frame batches: 8 row tiles for the 4x4 layers): a 256-wide N tile leaves 8 CTAs on
-  // 148 SMs, each walking the whole K serially.  Narrower N tiles (slices of the packed tile, 128B-swizzle layout
+  // few output rows (the actor's 64-frame batches: 8 row tiles for the 4x4 layers): a 128-wide N tile leaves 16 CTAs on
+  // 132 SMs, each walking the whole K serially.  Narrower N tiles (slices of the packed tile, 128B-swizzle layout
   // only) multiply the CTA count; the activation rows are re-gathered per slice out of L2.
   bool deep = false;
   if (g_umma_layout == 1) {
@@ -714,7 +680,6 @@ static int launch_igemm(ConvArgs a, int BN, cudaStream_t st) {
     case 32: HB_CONV_BN(32, 8); break;
     case 64: HB_CONV_BN(64, 8); break;
     case 128: HB_CONV_BN(128, 6); break;
-    case 256: HB_CONV_BN(256, 4); break;
     default:
       set_last_error("conv: unsupported N tile %d", BN);
       return HB200_ERR_UNSUPPORTED;
@@ -843,6 +808,14 @@ extern "C" int hb200_conv_wgrad(const hb200_bf16* x, const hb200_bf16* dy, float
   dim3 grid(mtiles, ntiles, nsplit);
   const size_t smem = (size_t)kStages * (kTileM * kChunkK * 2 + BN * kChunkK * 2) + 1024;
   cudaStream_t st = (cudaStream_t)stream;
+  // one partial per split, summed in split order into dw_acc (no floating-point atomics: deterministic)
+  const long long count = (long long)a.KW * s->co;
+  float* parts = nullptr;
+  int* tickets = nullptr;
+  rc = stream_workspace(st, (size_t)(nsplit + (nsplit < kReduceChunks ? nsplit : kReduceChunks)) * count, 0, &parts,
+                        &tickets);
+  if (rc) return rc;
+  a.dw = parts;
 #define HB_WG_CASE(bn)                                                                          \
   {                                                                                             \
     auto kern = conv_wgrad_kernel<bn>;                                                          \
@@ -853,7 +826,6 @@ extern "C" int hb200_conv_wgrad(const hb200_bf16* x, const hb200_bf16* dy, float
     case 32: HB_WG_CASE(32); break;
     case 64: HB_WG_CASE(64); break;
     case 128: HB_WG_CASE(128); break;
-    case 256: HB_WG_CASE(256); break;
     default:
       set_last_error("conv_wgrad: unsupported N tile %d", BN);
       return HB200_ERR_UNSUPPORTED;
@@ -861,7 +833,7 @@ extern "C" int hb200_conv_wgrad(const hb200_bf16* x, const hb200_bf16* dy, float
 #undef HB_WG_CASE
   HB_LAUNCH_OK();
   count_launch(1);
-  return HB200_OK;
+  return reduce_partials(parts, nsplit, count, count, dw_acc, parts + (size_t)nsplit * count, st);
 }
 
 extern "C" int hb200_pack_conv_weight(const float* w_oihw, hb200_bf16* w_packed,
@@ -912,28 +884,38 @@ extern "C" int hb200_unpack_conv_wgrad(const float* dw_acc, float* dw_oihw, int 
 extern "C" int hb200_umma_gemm_probe(const hb200_bf16* a, const hb200_bf16* b, float* d, int m, int n,
                                      int k, int layout, hb200_stream_t stream) {
   HB_CHECK_ARG(a && b && d, "probe: null pointer");
-  HB_CHECK_ARG(m % 128 == 0 && n % 16 == 0 && n >= 16 && n <= 256 && k % 64 == 0, "probe: bad dims");
-  // bit 4 / bit 5 of `layout`: operand A / B holds IEEE fp16 instead of bf16 (pins the mixed-format encoding)
-  const int a_fmt = (layout & 16) ? kFmtF16 : kFmtBF16, b_fmt = (layout & 32) ? kFmtF16 : kFmtBF16;
+  HB_CHECK_ARG(m % 128 == 0 && (n == 16 || n == 32 || n == 64 || n == 128) && k % 64 == 0, "probe: bad dims");
+  // bit 4 / bit 5 of `layout`: operand A / B holds IEEE fp16 instead of bf16; both operands must share one format
+  const bool a_f16 = (layout & 16) != 0, b_f16 = (layout & 32) != 0;
+  HB_CHECK_ARG(a_f16 == b_f16, "probe: the tensor core has no mixed fp16 x bf16 form");
   layout &= 15;
   HB_CHECK_ARG(layout >= 0 && layout <= 2, "probe: layout 0 (K-major no swizzle), 1 (K-major 128B), 2 (MN-major)");
   const size_t smem = (size_t)(kTileM + n) * kChunkK * 2 + 1024;
   cudaStream_t st = (cudaStream_t)stream;
   const __nv_bfloat16* A = (const __nv_bfloat16*)a;
   const __nv_bfloat16* B = (const __nv_bfloat16*)b;
-  if (layout == 0) {
-    auto kern = umma_probe_kernel<0, 0>;
-    HB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    kern<<<m / 128, 128, smem, st>>>(A, B, d, m, n, k, a_fmt, b_fmt);
-  } else if (layout == 1) {
-    auto kern = umma_probe_kernel<1, 0>;
-    HB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    kern<<<m / 128, 128, smem, st>>>(A, B, d, m, n, k, a_fmt, b_fmt);
-  } else {
-    auto kern = umma_probe_kernel<0, 1>;
-    HB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    kern<<<m / 128, 128, smem, st>>>(A, B, d, m, n, k, a_fmt, b_fmt);
+#define HB_PROBE(L, MN, NN, T)                                                                  \
+  {                                                                                             \
+    auto kern = umma_probe_kernel<L, MN, NN, T>;                                                \
+    HB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
+    kern<<<m / 128, 128, smem, st>>>(A, B, d, m, k);                                            \
   }
+#define HB_PROBE_N(L, MN, T)                    \
+  switch (n) {                                  \
+    case 16: HB_PROBE(L, MN, 16, T); break;     \
+    case 32: HB_PROBE(L, MN, 32, T); break;     \
+    case 64: HB_PROBE(L, MN, 64, T); break;     \
+    default: HB_PROBE(L, MN, 128, T); break;    \
+  }
+  if (layout == 0) {
+    if (a_f16) HB_PROBE_N(0, 0, kF16) else HB_PROBE_N(0, 0, kBF16)
+  } else if (layout == 1) {
+    if (a_f16) HB_PROBE_N(1, 0, kF16) else HB_PROBE_N(1, 0, kBF16)
+  } else {
+    if (a_f16) HB_PROBE_N(0, 1, kF16) else HB_PROBE_N(0, 1, kBF16)
+  }
+#undef HB_PROBE_N
+#undef HB_PROBE
   HB_LAUNCH_OK();
   count_launch(1);
   return HB200_OK;

@@ -3,12 +3,12 @@
 // over the space-to-depth input).
 //
 // The first-generation kernel (conv.cu) gathers an im2col tile per K chunk, so every input element
-// crosses L2 -> shared memory 9 times (ncu: lts 49 %, tensor pipe 4 %).  Here each CTA loads the
+// crosses L2 -> shared memory 9 times (L2-bound, the tensor pipe mostly idle).  Here each CTA loads the
 // (16+KH-1) x (8+KW-1) input halo of a 16x8 output tile ONCE into shared memory in the layout
 //
 //        offset(hy, cj, hx) = ((hy * C/8 + cj) * HW + hx) * 16 bytes        (16 B = 8 channels)
 //
-// and every filter tap is just a different tcgen05 shared-memory descriptor over that one buffer:
+// and every filter tap is just a different wgmma shared-memory descriptor over that one buffer:
 //   forward / dgrad (K-major A):  start = base + r*RP + s*16 + 2kk*P,  LBO = P (next 8 channels),
 //                                 SBO = RP (next output row = next 8-pixel core-matrix group)
 //   wgrad (MN-major A):           rows = (r, ci) with row-block stride P (because RP = C/8 * P the three
@@ -16,20 +16,20 @@
 // with P = HW*16, RP = (C/8)*P.  The no-swizzle descriptor mode is what makes this legal: shifting
 // the start address by one pixel (16 B) keeps every core matrix 8 x 16 B contiguous.
 //
-// CTAs are persistent (weights / accumulators stay resident across tiles); halo loads for tile i+1
-// (zero-filling cp.async: padding by predication) overlap the MMAs of tile i and the epilogue of
-// tile i-1 (double-buffered halo + double-buffered TMEM accumulators).
+// CTAs are persistent (weights stay resident across tiles); halo loads for tile i+1 (zero-filling
+// cp.async or TMA: padding by predication / out-of-bounds fill) overlap the MMAs and the epilogue of tile i.
+// One warpgroup owns the 128 x N accumulator of a tile in registers (wgmma.cuh).
 #include <cuda.h>
 #include <stdlib.h>
 
 #include "common.cuh"
-#include "umma.cuh"
+#include "wgmma.cuh"
 
 namespace hb200 {
 void count_launch(int n);
-using namespace umma;
+using namespace wg;
 
-constexpr int TH = 16, TW = 8;  // output tile: 16 rows x 8 cols = 128 pixels = UMMA M
+constexpr int TH = 16, TW = 8;  // output tile: 16 rows x 8 cols = 128 pixels = MMA M
 
 // transpose-reduce: each lane holds 16 partial sums v[i]; afterwards lane l holds the warp-wide sum of
 // v[l >> 1] (16 shuffles).  Lanes 2i and 2i+1 hold the same value.
@@ -131,10 +131,9 @@ struct HaloCfg {
   static constexpr int RP = CJ * P;             // bytes between halo rows
   static constexpr int HALO_BYTES = HH * RP;
   static constexpr int W_BYTES = KH * KW * C * N * 2;
-  static constexpr int TMEM_COLS = (2 * N) < 32 ? 32 : (2 * N);
   // Halo stages per CTA.  Two stages let one CTA overlap the next tile's loads with the current MMAs, but for
-  // C = N = 64 (72 KB of resident weights) that footprint (120 KB) leaves a single 128-thread CTA per SM -- ncu:
-  // 6 % occupancy, latency-bound.  One stage (97 KB) fits two CTAs per SM, which overlap each other instead.
+  // C = N = 64 (72 KB of resident weights) that footprint (120 KB) leaves a single 128-thread CTA per SM: latency-bound.
+  // One stage (97 KB) fits two CTAs per SM, which overlap each other instead.
   static constexpr int NBUF = (W_BYTES + 2 * HALO_BYTES > 110 * 1024) ? 1 : 2;
 };
 
@@ -158,7 +157,7 @@ __device__ __forceinline__ void load_halo(const __nv_bfloat16* __restrict__ x, u
 // Register-staged variant of load_halo for the weight-gradient kernels: coalesced LDG.128 (consecutive lanes walk the
 // channel chunks of consecutive pixels of a halo row = contiguous global bytes) into registers, later STS.128 into the
 // shifted-descriptor layout (bank-conflict free per 8-lane phase).  As LDGSTS the same copies cost 2 shared-memory
-// wavefronts per lane (ncu, profiles/r02_notes.md); staged through registers they cost ~8x fewer LSU cycles, and the
+// wavefronts per lane; staged through registers they cost ~8x fewer LSU cycles, and the
 // global latency hides behind the wait for the previous tile's MMAs.
 template <int C, int KH, int KW, int PAD, int ROWS, int NTHR>
 struct HaloRegs {
@@ -201,19 +200,12 @@ template <int C, int N, int KH, int KW, int PAD, int MODE>  // MODE 0: fwd (+sta
 __global__ void __launch_bounds__(128) conv_halo_kernel(const HaloArgs a) {
   using Cfg = HaloCfg<C, N, KH, KW, PAD>;
   extern __shared__ __align__(16) uint8_t smem_raw[];
-  __shared__ __align__(8) uint64_t mma_bar[2];
-  __shared__ uint32_t tmem_slot;
+  __shared__ float stage_buf[kStageFloats];
   const uint32_t sbase = (smem_u32(smem_raw) + 127u) & ~127u;
   const uint32_t s_w = sbase;
   const uint32_t s_halo0 = s_w + Cfg::W_BYTES;
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int tid = threadIdx.x, lane = tid & 31;
 
-  if (tid == 0) {
-    mbar_init(&mma_bar[0], 1);
-    mbar_init(&mma_bar[1], 1);
-    mbar_fence_init();
-  }
-  if (warp == 0) tmem_alloc(&tmem_slot, Cfg::TMEM_COLS);
   // weights: resident for the CTA's whole life
   {
     const uint4* src = reinterpret_cast<const uint4*>(a.wimg);
@@ -235,21 +227,16 @@ __global__ void __launch_bounds__(128) conv_halo_kernel(const HaloArgs a) {
     load_halo<C, KH, KW, PAD, Cfg::HH>(a.x, s_halo0, b, oh0, ow0, a.H, a.W);
   }
   cp_async_commit();  // group 0: weights + first halo
-  fence_before_sync();
-  __syncthreads();
-  fence_after_sync();
-  const uint32_t tmem_base = tmem_slot;
   // forward: fp16 input halo x fp16 weight image; dgrad: bf16 gradients x bf16 flipped / transposed image
-  constexpr uint32_t idesc = MODE == 0 ? make_idesc_f16(128, N, 0, 0, kFmtF16, kFmtF16) : make_idesc_bf16(128, N, 0, 0);
+  constexpr int kT = MODE == 0 ? kF16 : kBF16;
+  float acc_t[N];
 
   const int py = tid >> 3, px = tid & 7;  // this thread's output pixel within the tile (epilogue)
 
   constexpr int NBUF = Cfg::NBUF;
-  for (int it = 0; it <= my_n; ++it) {
+  for (int it = 0; it < my_n; ++it) {
     if (NBUF == 2) {
-      // (1) MMAs of tile it-1 are complete (frees halo stage (it+1)&1 and fills TMEM stage (it-1)&1)
-      if (it >= 1) mbar_wait(&mma_bar[(it - 1) & 1], ((it - 1) >> 1) & 1);
-      // (2) prefetch the halo of tile it+1
+      // prefetch the halo of tile it+1 into the stage tile it-1 used (its MMAs completed in the last iteration)
       if (it + 1 < my_n) {
         int b, oh0, ow0;
         tile_coords(first + (it + 1) * stride, b, oh0, ow0);
@@ -257,46 +244,46 @@ __global__ void __launch_bounds__(128) conv_halo_kernel(const HaloArgs a) {
       }
       cp_async_commit();
     }
-    // (3) halo of tile it has landed -> issue its MMAs
-    if (it < my_n) {
-      if (NBUF == 2) cp_async_wait<1>(); else cp_async_wait<0>();
-      fence_proxy_async_smem();
-      fence_before_sync();  // orders the previous iteration's tcgen05.ld (TMEM stage reuse) too
-      __syncthreads();
-      if (tid == 0) {
-        fence_after_sync();
-        const uint32_t sh = s_halo0 + (NBUF == 2 ? (it & 1) : 0) * Cfg::HALO_BYTES;
-        const uint32_t tacc = tmem_base + (uint32_t)((it & 1) * N);
-        uint32_t accum = 0;
+    // halo of tile it has landed -> its MMAs
+    if (NBUF == 2) cp_async_wait<1>(); else cp_async_wait<0>();
+    fence_proxy_async_smem();
+    __syncthreads();
+    {
+      const uint32_t sh = s_halo0 + (NBUF == 2 ? (it & 1) : 0) * Cfg::HALO_BYTES;
+      wgmma_fence();
+      uint32_t accum = 0;
 #pragma unroll
-        for (int r = 0; r < KH; ++r)
+      for (int r = 0; r < KH; ++r)
 #pragma unroll
-          for (int s = 0; s < KW; ++s)
+        for (int s = 0; s < KW; ++s)
 #pragma unroll
-            for (int kk = 0; kk < C / 16; ++kk) {
-              const uint64_t da = make_smem_desc(sh + r * Cfg::RP + s * 16 + 2 * kk * Cfg::P, Cfg::P, Cfg::RP, kNoSwizzle);
-              const uint64_t db = make_smem_desc(s_w + (r * KW + s) * (C * N * 2) + 2 * kk * (N * 16), N * 16, 128, kNoSwizzle);
-              mma_bf16_ss(tacc, da, db, idesc, accum);
-              accum = 1;
-            }
-        mma_commit(&mma_bar[it & 1]);
-      }
+          for (int kk = 0; kk < C / 16; ++kk) {
+            const uint64_t da = make_smem_desc(sh + r * Cfg::RP + s * 16 + 2 * kk * Cfg::P, Cfg::P, Cfg::RP, kNoSwizzle);
+            const uint64_t db = make_smem_desc(s_w + (r * KW + s) * (C * N * 2) + 2 * kk * (N * 16), N * 16, 128, kNoSwizzle);
+            mma128<N, kT>(acc_t, da, 8 * Cfg::RP, db, accum);
+            accum = 1;
+          }
+      wgmma_commit();
+      wgmma_wait<0>();
+      acc_fence(acc_t);
     }
-    // (4) epilogue of tile it-1 (overlaps the tensor core working on tile it)
-    if (it >= 1) {
-      fence_after_sync();
+    // single halo stage: the MMAs of tile it have consumed it -> the next tile loads during this epilogue
+    if (NBUF == 1) {
+      if (it + 1 < my_n) {
+        int b, oh0, ow0;
+        tile_coords(first + (it + 1) * stride, b, oh0, ow0);
+        load_halo<C, KH, KW, PAD, Cfg::HH>(a.x, s_halo0, b, oh0, ow0, a.H, a.W);
+      }
+      cp_async_commit();
+    }
+    {   // epilogue of tile it
       int b, oh0, ow0;
-      tile_coords(first + (it - 1) * stride, b, oh0, ow0);
-      const uint32_t taddr = tmem_base + ((uint32_t)(warp * 32) << 16) + (uint32_t)(((it - 1) & 1) * N);
+      tile_coords(first + it * stride, b, oh0, ow0);
       const size_t pix = ((size_t)b * a.H + oh0 + py) * a.W + ow0 + px;
-#pragma unroll 1
-      for (int col0 = 0; col0 < N; col0 += 32) {
-        uint32_t rr[32];
-        tmem_ld32(taddr + col0, rr);
-        tmem_ld_wait();
-        float acc[32];
 #pragma unroll
-        for (int j = 0; j < 32; ++j) acc[j] = __uint_as_float(rr[j]);
+      for (int col0 = 0; col0 < N; col0 += 32) {
+        float acc[32];
+        acc_row32(acc_t, col0, stage_buf, acc);
         if (MODE == 0 && a.stats != nullptr) {
           // per (frame, group) sum / sum-of-squares of this 32-column slab over the warp's 32 pixels:
           // pairwise channel sums, then a transpose-reduce (16 + 16 shuffles instead of 2 x 16 x 5)
@@ -345,31 +332,22 @@ __global__ void __launch_bounds__(128) conv_halo_kernel(const HaloArgs a) {
         }
       }
     }
-    if (NBUF == 1 && it < my_n) {
-      // single halo stage: the MMAs of tile it must have consumed it before the next tile's loads overwrite it
-      // (the other CTA on this SM covers the gap); this is also the completion the next epilogue needs
-      mbar_wait(&mma_bar[it & 1], (it >> 1) & 1);
-      if (it + 1 < my_n) {
-        int b, oh0, ow0;
-        tile_coords(first + (it + 1) * stride, b, oh0, ow0);
-        load_halo<C, KH, KW, PAD, Cfg::HH>(a.x, s_halo0, b, oh0, ow0, a.H, a.W);
-      }
-      cp_async_commit();
-    }
   }
-  fence_before_sync();
-  __syncthreads();
-  if (warp == 0) tmem_dealloc(tmem_base, Cfg::TMEM_COLS);
 }
 
 // ------------------------------------------------------------------------------------------
 // weight gradient on the same halo buffer.  rows = (r, ci) [vertical taps form one affine M dim],
 // one accumulator per horizontal tap s and per 128-row M tile; K = output pixels.
 // ------------------------------------------------------------------------------------------
+// ring depth of conv_halo_wgrad_kernel: 4 stages where they fit beside the 17 KB accumulator transpose buffer, else 3
+constexpr int halo_wgrad_stages(int xmode, int c, int stage_bytes) {
+  return (xmode != 0 && c >= 64) ? (4 * stage_bytes <= 200 * 1024 ? 4 : 3) : 2;
+}
+
 struct HaloWgradArgs {
   const __nv_bfloat16* x;   // [B,H,W,C]
   const __nv_bfloat16* dy;  // [B,H,W,N]
-  float* dw;                // [(r*KW+s)*C + ci][N]  (same accumulator layout as conv_wgrad_kernel)
+  float* dw;                // partials [blockIdx.x][(r*KW+s)*C + ci][N], summed in order by reduce_partials
   int B, H, W, ntiles;
 };
 
@@ -391,32 +369,29 @@ conv_halo_wgrad_kernel(const HaloWgradArgs a, const __grid_constant__ CUtensorMa
   constexpr int HALO_BYTES = HROWS * RP;
   constexpr int DY_BYTES = 128 * N * 2;                    // [pixel][N channels]: one swizzled row per pixel (TMA)
   constexpr int STAGE = (DY_BYTES + HALO_BYTES + 1023) / 1024 * 1024;   // dy tile first: swizzle atoms need 1024-byte alignment
-  // Ring depth.  With the x halo AND the dy tile arriving by TMA the loop is one thread: wait tile, issue MMAs; two stages
-  // exposed the ~1.5 us load latency once per tile (the MMAs of a 32-channel tile take 0.2 us): prefetch NSW-1 tiles ahead.
-  // Measured (4096 frames): 64 channels 133 -> 122 us, stride-2 view (128 virtual channels) 107 -> 99 us -- configurations
-  // that are one CTA per SM anyway (TMEM / shared memory); 32 channels 159 -> 171 us and the stem 650 -> 713 us lose more
-  // from the halved CTA count (each CTA = one MMA-issuing thread) than they gain: two stages there.
-  constexpr int NSW = (XMODE != 0 && C >= 64) ? 4 : 2;
+  // Ring depth.  With the x halo AND the dy tile arriving by TMA, two stages expose the load latency of a tile once per
+  // tile (its MMAs are much shorter): the wide configurations, one CTA per SM anyway (shared memory), prefetch NSW-1 tiles
+  // ahead; the 32-channel layers and the stem keep two stages and more CTAs per SM instead.
+  constexpr int NSW = halo_wgrad_stages(XMODE, C, STAGE);
+  // accumulators (s, mt) of 128 rows x N: a CTA holds APC of them in registers (<= 128 columns), blockIdx.y picks the group
   constexpr int NACC = KW * MT;
-  constexpr int TCOLS_RAW = NACC * N;
-  constexpr int TMEM_COLS = TCOLS_RAW <= 32 ? 32 : TCOLS_RAW <= 64 ? 64 : TCOLS_RAW <= 128 ? 128 : TCOLS_RAW <= 256 ? 256 : 512;
-  static_assert(TCOLS_RAW <= 512, "accumulators exceed TMEM");
+  constexpr int APC = NACC * N <= 128 ? NACC : 128 / N;
+  static_assert(NACC % APC == 0, "accumulator groups");
   static_assert(N == 32 || N == 64, "dy rows are 64 / 128 bytes: SWIZZLE_64B / SWIZZLE_128B");
   extern __shared__ __align__(16) uint8_t smem_raw[];
-  __shared__ __align__(8) uint64_t mma_bar[NSW];
   __shared__ __align__(8) uint64_t dy_bar[NSW];
-  __shared__ uint32_t tmem_slot;
+  __shared__ float stage_buf[kStageFloats];
   const uint32_t sbase = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const int tid = threadIdx.x, warp = tid >> 5;
+  const int tid = threadIdx.x;
+  const int grp = blockIdx.y;
   const CUtensorMap* const tmap_p = &tmap_dy;   // param-space address (never through a by-reference lambda capture)
   const CUtensorMap* const tmap_xp = &tmap_x;
 
   if (tid == 0) {
 #pragma unroll
-    for (int i = 0; i < NSW; ++i) { mbar_init(&mma_bar[i], 1); mbar_init(&dy_bar[i], 1); }
+    for (int i = 0; i < NSW; ++i) mbar_init(&dy_bar[i], 1);
     mbar_fence_init();
   }
-  if (warp == 0) tmem_alloc(&tmem_slot, TMEM_COLS);
   // the padding halo rows are read by the (discarded) padding M rows: keep them finite
   for (int st = 0; st < NSW; ++st)
     for (int v = tid; v < (HROWS - HROWS_LOAD) * RP / 16; v += 128) {
@@ -434,8 +409,8 @@ conv_halo_wgrad_kernel(const HaloWgradArgs a, const __grid_constant__ CUtensorMa
   // 8 x 16 pixels) into the MN-major swizzled layout -- as LDGSTS it was a transpose (pixel-major tensor -> channel-chunk-
   // major rows), 2 shared-memory wavefronts per 16-byte copy, which made this kernel LSU-bound (see the small-image
   // kernel below).
-  // Register staging pays while the halo is <= 8 vectors per thread (C <= 32: 0.211 -> 0.165 ms per layer, stem 0.79 ->
-  // 0.67); for C = 64 (12 vectors, 128 registers) the lost occupancy costs more than the LDGSTS wavefronts: cp.async there.
+  // Register staging pays while the halo is <= 8 vectors per thread (C <= 32, the stem); for C = 64 (12 vectors, 128
+  // registers) the lost occupancy costs more than the LDGSTS wavefronts: cp.async there.
   constexpr bool kRegStage = XMODE == 0 && HROWS_LOAD * CJ * HWD <= 128 * 8;
   HaloRegs<C, KH, KW, PAD, kRegStage ? HROWS_LOAD : 1, 128> xr;   // the x halo of the NEXT tile, in flight in registers
   auto fetch_x = [&](int tile) {
@@ -468,122 +443,95 @@ conv_halo_wgrad_kernel(const HaloWgradArgs a, const __grid_constant__ CUtensorMa
   }
   cp_async_commit();
   fence_proxy_async_smem();
-  fence_before_sync();
   __syncthreads();
-  fence_after_sync();
-  const uint32_t tmem_base = tmem_slot;
   // A = bf16 twin of the forward activations (halo), B = output gradients (bf16); mixed fp16 x bf16 is not legal
-  constexpr uint32_t idesc = make_idesc_bf16(128, N, 1, 1);
+  float acc_w[APC][N];
+  auto mma_tile = [&](int it, uint32_t sd) {   // all 128 threads; returns with the MMAs complete
+    const uint32_t sh = sd + DY_BYTES;
+    wgmma_fence();
+#pragma unroll
+    for (int l = 0; l < APC; ++l) {
+      const int ai = grp * APC + l, s = ai / MT, mt = ai % MT;
+#pragma unroll
+      for (int ks = 0; ks < TH / 2; ++ks) {
+        // A: M = row blocks (stride P), K = 16 pixels = tile rows 2ks, 2ks+1 (stride RP)
+        const uint64_t da = make_smem_desc(sh + 2 * ks * RP + s * 16 + mt * 16 * P, RP, P, kNoSwizzle);
+        // B: MN-major swizzled rows (one pixel = N channels = 64 / 128 bytes); K16 = 2 groups of 8 rows
+        const uint64_t db = make_smem_desc(sd + ks * (16 * N * 2), 0, 8 * N * 2, N == 64 ? kSwizzle128B : kSwizzle64B);
+        mma128<N, kBF16, 1, 1>(acc_w[l], da, 8 * P, db, (it > 0 || ks > 0) ? 1u : 0u);
+      }
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+  };
 
   if (XMODE != 0) {
-    // both operands by TMA: ONE thread runs the whole pipeline, NSW-1 tiles of loads ahead of the tensor core
-    if (tid == 0) {
+    // both operands by TMA: thread 0 keeps NSW-1 tiles of loads ahead of the tensor core
+    if (tid == 0)
       for (int p = 0; p < NSW - 1 && p < my_n; ++p) commit_tile(first + p * stride, p);
-      for (int it = 0; it < my_n; ++it) {
-        const int nxt = it + NSW - 1;
-        if (nxt < my_n) {
-          if (nxt >= NSW) mbar_wait(&mma_bar[nxt % NSW], ((nxt / NSW) - 1) & 1);   // the MMAs that read this stage
-          commit_tile(first + nxt * stride, nxt % NSW);
-        }
-        mbar_wait(&dy_bar[it % NSW], (it / NSW) & 1);
-        fence_after_sync();
-        const uint32_t sd = sbase + (it % NSW) * STAGE;
-        const uint32_t sh = sd + DY_BYTES;
-#pragma unroll
-      for (int s = 0; s < KW; ++s)
-#pragma unroll
-        for (int mt = 0; mt < MT; ++mt)
-#pragma unroll
-          for (int ks = 0; ks < TH / 2; ++ks) {
-            // A: M = row blocks (stride P), K = 16 pixels = tile rows 2ks, 2ks+1 (stride RP)
-            const uint64_t da = make_smem_desc(sh + 2 * ks * RP + s * 16 + mt * 16 * P, RP, P, kNoSwizzle);
-            // B: MN-major swizzled rows (one pixel = N channels = 64 / 128 bytes); K16 = 2 groups of 8 rows
-            const uint64_t db = make_smem_desc(sd + ks * (16 * N * 2), 0, 8 * N * 2, N == 64 ? kSwizzle128B : kSwizzle64B);
-            mma_bf16_ss(tmem_base + (uint32_t)((s * MT + mt) * N), da, db, idesc, (it > 0 || ks > 0) ? 1u : 0u);
-          }
-        mma_commit(&mma_bar[it % NSW]);
-      }
+    for (int it = 0; it < my_n; ++it) {
+      const int nxt = it + NSW - 1;   // its stage was read by the MMAs of tile it-1, complete
+      if (tid == 0 && nxt < my_n) commit_tile(first + nxt * stride, nxt % NSW);
+      mbar_wait(&dy_bar[it % NSW], (it / NSW) & 1);
+      mma_tile(it, sbase + (it % NSW) * STAGE);
     }
-    __syncthreads();
   } else {
-  for (int it = 0; it < my_n; ++it) {
+    for (int it = 0; it < my_n; ++it) {
       const bool more = it + 1 < my_n;
       if (more) fetch_x(first + (it + 1) * stride);                 // global loads in flight ...
-      if (it >= 1) mbar_wait(&mma_bar[(it - 1) & 1], ((it - 1) >> 1) & 1);   // ... while the stage drains
-      if (more) commit_tile(first + (it + 1) * stride, (it + 1) & 1);
+      if (more) commit_tile(first + (it + 1) * stride, (it + 1) & 1);   // ... into the stage tile it-1 used
       cp_async_commit();
       cp_async_wait<1>();         // cp.async variant: this thread's copies of tile it (issued an iteration ago)
-      fence_proxy_async_smem();   // st.shared / cp.async (generic proxy) -> tcgen05 (async proxy)
+      fence_proxy_async_smem();   // st.shared / cp.async (generic proxy) -> wgmma (async proxy)
       __syncthreads();
-      if (tid == 0) {
-        mbar_wait(&dy_bar[it & 1], (it >> 1) & 1);   // the TMA'd dy tile
-        fence_after_sync();
-        const uint32_t sd = sbase + (it & 1) * STAGE;
-        const uint32_t sh = sd + DY_BYTES;
-#pragma unroll
-        for (int s = 0; s < KW; ++s)
-#pragma unroll
-          for (int mt = 0; mt < MT; ++mt)
-#pragma unroll
-            for (int ks = 0; ks < TH / 2; ++ks) {
-              // A: M = row blocks (stride P), K = 16 pixels = tile rows 2ks, 2ks+1 (stride RP)
-              const uint64_t da = make_smem_desc(sh + 2 * ks * RP + s * 16 + mt * 16 * P, RP, P, kNoSwizzle);
-              // B: MN-major swizzled rows (one pixel = N channels = 64 / 128 bytes); K16 = 2 groups of 8 rows
-              const uint64_t db = make_smem_desc(sd + ks * (16 * N * 2), 0, 8 * N * 2, N == 64 ? kSwizzle128B : kSwizzle64B);
-              mma_bf16_ss(tmem_base + (uint32_t)((s * MT + mt) * N), da, db, idesc, (it > 0 || ks > 0) ? 1u : 0u);
-            }
-        mma_commit(&mma_bar[it & 1]);
-      }
+      mbar_wait(&dy_bar[it & 1], (it >> 1) & 1);   // the TMA'd dy tile
+      mma_tile(it, sbase + (it & 1) * STAGE);
     }
   }
-  if (my_n > 0) {
-    mbar_wait(&mma_bar[(my_n - 1) % NSW], ((my_n - 1) / NSW) & 1);
-    fence_after_sync();
-    const uint32_t taddr = tmem_base + ((uint32_t)(warp * 32) << 16);
-#pragma unroll 1
-    for (int acc = 0; acc < NACC; ++acc) {
-      const int s = acc / MT, mt = acc % MT;
+  {   // a worker without tiles still writes its (zero) partial
+#pragma unroll
+    for (int l = 0; l < APC; ++l) {
+      if (my_n == 0) {
+#pragma unroll
+        for (int j = 0; j < N; ++j) acc_w[l][j] = 0.f;
+      }
+      acc_fence(acc_w[l]);
+      const int ai = grp * APC + l, s = ai / MT, mt = ai % MT;
       const int blk = mt * 16 + (tid >> 3);       // row block (r, cj)
       const int r = blk / CJ, cj = blk % CJ;
       const bool ok = r < KH;
       const size_t row = (size_t)(r * KW + s) * C + cj * 8 + (tid & 7);
-#pragma unroll 1
-      for (int col0 = 0; col0 < N; col0 += 32) {
-        uint32_t rr[32];
-        tmem_ld32(taddr + (uint32_t)(acc * N + col0), rr);
-        tmem_ld_wait();
-        if (ok) {
-          float* dst = a.dw + row * N + col0;
 #pragma unroll
-          for (int j = 0; j < 32; j += 4)
-            red_add_v4(dst + j, __uint_as_float(rr[j]), __uint_as_float(rr[j + 1]), __uint_as_float(rr[j + 2]),
-                       __uint_as_float(rr[j + 3]));
+      for (int col0 = 0; col0 < N; col0 += 32) {
+        float rr[32];
+        acc_row32(acc_w[l], col0, stage_buf, rr);
+        if (ok) {
+          float* dst = a.dw + ((size_t)blockIdx.x * (KH * KW * C) + row) * N + col0;
+#pragma unroll
+          for (int j = 0; j < 32; j += 4) *reinterpret_cast<float4*>(dst + j) = make_float4(rr[j], rr[j + 1], rr[j + 2], rr[j + 3]);
         }
       }
     }
   }
-  fence_before_sync();
-  __syncthreads();
-  if (warp == 0) tmem_dealloc(tmem_base, TMEM_COLS);
 }
 
 
 // ------------------------------------------------------------------------------------------
 // weight gradient of the 3x3 pad-1 stride-1 convs on SMALL images (8x8: layer3, 4x4: layer4 / compression).
 // The gather kernel (conv.cu) re-reads x once per tap and dy once per 128-row M tile through L2 (1.2 GB per launch
-// for a 128->128 layer: L2-gather-bound at ~10 % of the tensor roofline).  Here the halo scheme of the kernel above
+// for a 128->128 layer: L2-gather-bound, far below the tensor roofline).  Here the halo scheme of the kernel above
 // is applied to a tile made of SEVERAL images: a 16x8 output tile = 16/IMG images stacked vertically, each with its
 // own zero-padding rows in the halo buffer (and, for 4x4 images, 4 zero "virtual" pixels per 8-pixel row whose dy is
 // zero), so x is loaded once per (channel slice) and every tap is a shifted descriptor.  Channels are sliced to keep
-// the 9 accumulators inside TMEM: a CTA owns 32 input channels (the three vertical taps x 32 channels = 96 rows of
-// one M = 128 tile) and NS output channels: accumulators = 3 horizontal taps x NS columns (NS = 128 -> 384).
-// grid = (tile workers, Ci/32 * Co/NS slices); results are accumulated into dw with vector red.add.
+// the accumulator in registers: a CTA owns 32 input channels (the three vertical taps x 32 channels = 96 rows of
+// one M = 128 tile), NS output channels and ONE horizontal tap s (a 128 x NS accumulator).
+// grid = (tile workers, Ci/32 * Co/NS slices x 3 taps); results are accumulated into dw with vector red.add.
 // ------------------------------------------------------------------------------------------
 constexpr int kSmallWgradStages = 3;
 struct HaloWgradSmallArgs {
   const grad_t* x;    // [B, IMG, IMG, Ci]  bf16 twin of the forward activation
   const grad_t* dy;   // [B, IMG, IMG, Co]  bf16
-  float* dw;          // [(r*3+s)*Ci + ci][Co]
+  float* dw;          // partials [blockIdx.x][(r*3+s)*Ci + ci][Co], summed in order by reduce_partials
   int B, Ci, Co, ntiles;
 };
 
@@ -602,32 +550,29 @@ conv_halo_wgrad_small_kernel(const HaloWgradSmallArgs a, const __grid_constant__
   constexpr int DY_BYTES = NB * 128 * 128;      // [block][pixel][128 B], TMA SWIZZLE_128B
   constexpr int STAGE = HALO_BYTES + DY_BYTES;
   constexpr int NST = kSmallWgradStages;        // 3-deep ring: the loads of tile it+2 overlap the MMAs of tiles it, it+1
-  constexpr int TCOLS_RAW = KW * NS;
-  constexpr int TMEM_COLS = TCOLS_RAW <= 128 ? 128 : TCOLS_RAW <= 256 ? 256 : 512;
-  static_assert(TCOLS_RAW <= 512, "accumulators exceed TMEM");
+  static_assert(NS <= 128, "one 128 x NS accumulator per CTA");
   extern __shared__ __align__(16) uint8_t smem_raw[];
-  __shared__ __align__(8) uint64_t mma_bar[NST];
   __shared__ __align__(8) uint64_t dy_bar[NST];
-  __shared__ uint32_t tmem_slot;
+  __shared__ float stage_buf[kStageFloats];
   const uint32_t sbase = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const int tid = threadIdx.x, warp = tid >> 5;
   const int nsl = a.Co / NS;
-  const int c_off = (blockIdx.y / nsl) * 32, n_off = (blockIdx.y % nsl) * NS;
+  const int s_tap = blockIdx.y % KW, slice = blockIdx.y / KW;   // horizontal tap of this CTA's accumulator
+  const int c_off = (slice / nsl) * 32, n_off = (slice % nsl) * NS;
   const CUtensorMap* const tmap_p = &tmap_dy;   // param-space address (see conv_halo_tma_kernel)
 
   if (tid == 0) {
 #pragma unroll
-    for (int i = 0; i < NST; ++i) { mbar_init(&mma_bar[i], 1); mbar_init(&dy_bar[i], 1); }
+    for (int i = 0; i < NST; ++i) mbar_init(&dy_bar[i], 1);
     mbar_fence_init();
   }
-  if (warp == 0) tmem_alloc(&tmem_slot, TMEM_COLS);
   // rows beyond the loaded ones are read by the (discarded) padding M rows: keep them finite
   for (int st = 0; st < NST; ++st)
     for (int v = tid; v < (HROWS_A - HROWS_LOAD) * RP / 16; v += 128) {
       const uint32_t addr = sbase + st * STAGE + HROWS_LOAD * RP + v * 16;
       asm volatile("st.shared.v4.b32 [%0], {%1,%1,%1,%1};" ::"r"(addr), "r"(0u) : "memory");
     }
-  // Operand traffic.  ncu on the all-cp.async version: every LDGSTS of the dy tile cost 64 shared-memory wavefronts
+  // Operand traffic.  In an all-cp.async version every LDGSTS of the dy tile costs 64 shared-memory wavefronts
   // (ideal 8) -- a 16-byte copy only coalesces with its neighbours when 8 lanes are contiguous in BOTH global and
   // shared memory, and the MN-major no-swizzle layout ([channel chunk][pixel][16 B]) is a transpose of the pixel-major
   // tensor; 5700 LSU cycles per tile against 1536 tensor cycles.  The dy tile now arrives by TMA (box = 64 channels x
@@ -693,11 +638,8 @@ conv_halo_wgrad_small_kernel(const HaloWgradSmallArgs a, const __grid_constant__
     }
   }
   fence_proxy_async_smem();
-  fence_before_sync();
   __syncthreads();
-  fence_after_sync();
-  const uint32_t tmem_base = tmem_slot;
-  constexpr uint32_t idesc = make_idesc_bf16(128, NS, 1, 1);
+  float acc_t[NS];
 
   for (int it = 0; it < my_n; ++it) {
     const int st = it % NST;
@@ -705,61 +647,51 @@ conv_halo_wgrad_small_kernel(const HaloWgradSmallArgs a, const __grid_constant__
     if (nt < my_n) fetch_x(first + nt * stride);   // its x halo: global loads in flight from here on
     fence_proxy_async_smem();        // x halo of tile it was stored (st.shared) an iteration ago
     __syncthreads();
-    if (tid == 0) {
-      mbar_wait(&dy_bar[st], (it / NST) & 1);   // the TMA'd dy tile
-      fence_after_sync();
+    mbar_wait(&dy_bar[st], (it / NST) & 1);   // the TMA'd dy tile
+    {
       const uint32_t sh = sbase + st * STAGE;
       const uint32_t sd = sh + HALO_BYTES;
+      wgmma_fence();
 #pragma unroll
-      for (int s = 0; s < KW; ++s)
-#pragma unroll
-        for (int ks = 0; ks < TH / 2; ++ks) {
-          // K16 = tile rows 2ks, 2ks+1 (never straddle an image: IMG is even) -> halo rows hb, hb+1 (+ tap r in M)
-          const int hb = ((2 * ks) / IMG) * RPI + (2 * ks) % IMG;
-          const uint64_t da = make_smem_desc(sh + hb * RP + s * 16, RP, P, kNoSwizzle);
-          // B: MN-major, 128-byte swizzle: rows = pixels (K), 128 B = 64 channels; K16 = 2 groups of 8 rows (1024 B each);
-          // LBO = next 64-channel block (128 rows x 128 B), SBO = next 8-row group
-          const uint64_t db = make_smem_desc(sd + ks * 2048, 128 * 128, 1024, kSwizzle128B);
-          mma_bf16_ss(tmem_base + (uint32_t)(s * NS), da, db, idesc, (it > 0 || ks > 0) ? 1u : 0u);
-        }
-      mma_commit(&mma_bar[st]);
+      for (int ks = 0; ks < TH / 2; ++ks) {
+        // K16 = tile rows 2ks, 2ks+1 (never straddle an image: IMG is even) -> halo rows hb, hb+1 (+ tap r in M)
+        const int hb = ((2 * ks) / IMG) * RPI + (2 * ks) % IMG;
+        const uint64_t da = make_smem_desc(sh + hb * RP + s_tap * 16, RP, P, kNoSwizzle);
+        // B: MN-major, 128-byte swizzle: rows = pixels (K), 128 B = 64 channels; K16 = 2 groups of 8 rows (1024 B each);
+        // LBO = next 64-channel block (128 rows x 128 B), SBO = next 8-row group
+        const uint64_t db = make_smem_desc(sd + ks * 2048, 128 * 128, 1024, kSwizzle128B);
+        mma128<NS, kBF16, 1, 1>(acc_t, da, 8 * P, db, (it > 0 || ks > 0) ? 1u : 0u);
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
     }
-    // refill the stage tile it-1 used with tile it+NST-1 (its MMAs were queued before tile it's, which now keep the
-    // tensor core busy while we wait and load)
+    // refill the stage tile it-1 used (its MMAs are complete) with tile it+NST-1
     if (nt < my_n) {
-      if (it >= 1) mbar_wait(&mma_bar[(it - 1) % NST], ((it - 1) / NST) & 1);
       store_x(nt % NST);
       if (tid == 0) load_dy(first + nt * stride, nt % NST);
     }
   }
-  if (my_n > 0) {
-    mbar_wait(&mma_bar[(my_n - 1) % NST], ((my_n - 1) / NST) & 1);
-    fence_after_sync();
-    const uint32_t taddr = tmem_base + ((uint32_t)(warp * 32) << 16);
+  {   // a worker without tiles still writes its (zero) partial
+    if (my_n == 0) {
+#pragma unroll
+      for (int j = 0; j < NS; ++j) acc_t[j] = 0.f;
+    }
+    acc_fence(acc_t);
     const int blk = tid >> 3;                  // row block (r, cj)
     const int r = blk / CJ, cj = blk % CJ;
     const bool ok = r < KH;
-#pragma unroll 1
-    for (int s = 0; s < KW; ++s) {
-      const size_t row = (size_t)(r * KW + s) * a.Ci + c_off + cj * 8 + (tid & 7);
-#pragma unroll 1
-      for (int col0 = 0; col0 < NS; col0 += 32) {
-        uint32_t rr[32];
-        tmem_ld32(taddr + (uint32_t)(s * NS + col0), rr);
-        tmem_ld_wait();
-        if (ok) {
-          float* dst = a.dw + row * a.Co + n_off + col0;
+    const size_t row = (size_t)(r * KW + s_tap) * a.Ci + c_off + cj * 8 + (tid & 7);
 #pragma unroll
-          for (int j = 0; j < 32; j += 4)
-            red_add_v4(dst + j, __uint_as_float(rr[j]), __uint_as_float(rr[j + 1]), __uint_as_float(rr[j + 2]),
-                       __uint_as_float(rr[j + 3]));
-        }
+    for (int col0 = 0; col0 < NS; col0 += 32) {
+      float rr[32];
+      acc_row32(acc_t, col0, stage_buf, rr);
+      if (ok) {
+        float* dst = a.dw + ((size_t)blockIdx.x * 9 * a.Ci + row) * a.Co + n_off + col0;
+#pragma unroll
+        for (int j = 0; j < 32; j += 4) *reinterpret_cast<float4*>(dst + j) = make_float4(rr[j], rr[j + 1], rr[j + 2], rr[j + 3]);
       }
     }
   }
-  fence_before_sync();
-  __syncthreads();
-  if (warp == 0) tmem_dealloc(tmem_base, TMEM_COLS);
 }
 
 // ---- weight image for the halo kernels: [tap][C/8][N][8] bf16 ---------------------------------
@@ -806,16 +738,16 @@ __global__ void unpack_stem_wgrad_kernel(const float* __restrict__ acc, float* _
   }
 }
 
-// resident CTAs per SM from static limits (registers, shared memory, TMEM columns); cached per kernel
+// resident CTAs per SM from static limits (registers, shared memory); cached per kernel
 // ------------------------------------------------------------------------------------------
-// DEFAULT for the 32-channel 3x3 layers and the stem since round 2 (HB200_NO_HALO_TMA=1 falls back to the cp.async
-// kernel above): the same persistent forward / dgrad kernel with the halo loaded by TMA.  One thread issues C/8
+// The same persistent forward / dgrad kernel with the halo loaded by TMA (HB200_NO_HALO_TMA=1 falls back to the cp.async
+// kernel above).  One thread issues C/8
 // `cp.async.bulk.tensor.4d` box copies per tile (box = {8 channels, halo width, halo height, 1 frame}; the conv
 // padding is the TMA unit's out-of-bounds zero fill) that complete on an mbarrier, instead of ~6 predicated
-// cp.async per thread -- the address / predicate arithmetic that makes conv_halo_kernel<32,32> issue-bound
-// (profiles/r01f_ncu_top_kernels.md).  The box lands as [cj][hy][hx][8 ch], so the K-major descriptors become
+// cp.async per thread -- the address / predicate arithmetic that makes conv_halo_kernel<32,32> issue-bound.
+// The box lands as [cj][hy][hx][8 ch], so the K-major descriptors become
 //   start = stage + 2kk*SLAB + r*HWD*16 + s*16,   LBO = SLAB (next 8 channels),   SBO = HWD*16 (next tile row).
-// Only the MMA-issuing thread waits for the load; the epilogue warps never touch the halo.
+// The warpgroup waits for the load on the stage's mbarrier before it issues the tile's MMAs.
 // ------------------------------------------------------------------------------------------
 
 template <int C, int N, int KH, int KW, int PAD, int MODE>
@@ -830,22 +762,18 @@ conv_halo_tma_kernel(const HaloArgs a, const __grid_constant__ CUtensorMap tmap)
   // the gap -- like conv_halo_kernel, minus the 2880 LSU cycles per tile its cp.async halo gather costs
   constexpr int NB = (Cfg::W_BYTES + 2 * (int)STAGE > 110 * 1024) ? 1 : 2;
   extern __shared__ __align__(16) uint8_t smem_raw[];
-  __shared__ __align__(8) uint64_t mma_bar[2];
   __shared__ __align__(8) uint64_t ld_bar[2];
-  __shared__ uint32_t tmem_slot;
+  __shared__ float stage_buf[kStageFloats];
   const uint32_t sbase = (smem_u32(smem_raw) + 127u) & ~127u;
   const uint32_t s_w = sbase;
   const uint32_t s_halo0 = s_w + Cfg::W_BYTES;   // W_BYTES is a multiple of 128
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int tid = threadIdx.x, lane = tid & 31;
 
   if (tid == 0) {
-    mbar_init(&mma_bar[0], 1);
-    mbar_init(&mma_bar[1], 1);
     mbar_init(&ld_bar[0], 1);
     mbar_init(&ld_bar[1], 1);
     mbar_fence_init();
   }
-  if (warp == 0) tmem_alloc(&tmem_slot, Cfg::TMEM_COLS);
   {
     const uint4* src = reinterpret_cast<const uint4*>(a.wimg);
     for (int v = tid; v < Cfg::W_BYTES / 16; v += 128) cp_async16(s_w + (uint32_t)v * 16, src + v, true);
@@ -874,61 +802,49 @@ conv_halo_tma_kernel(const HaloArgs a, const __grid_constant__ CUtensorMap tmap)
   };
   const int first = blockIdx.x, stride = gridDim.x;
   const int my_n = first < a.ntiles ? (a.ntiles - first + stride - 1) / stride : 0;
+  __syncthreads();   // barriers initialised
   if (tid == 0 && my_n > 0) issue_halo(first, 0);
   cp_async_wait<0>();          // weights
-  fence_proxy_async_smem();    // cp.async (generic proxy) -> tcgen05 (async proxy)
-  fence_before_sync();
+  fence_proxy_async_smem();    // cp.async (generic proxy) -> wgmma (async proxy)
   __syncthreads();
-  fence_after_sync();
-  const uint32_t tmem_base = tmem_slot;
   // forward: fp16 input halo x fp16 weight image; dgrad: bf16 gradients x bf16 flipped / transposed image
-  constexpr uint32_t idesc = MODE == 0 ? make_idesc_f16(128, N, 0, 0, kFmtF16, kFmtF16) : make_idesc_bf16(128, N, 0, 0);
+  constexpr int kT = MODE == 0 ? kF16 : kBF16;
+  float acc_t[N];
   const int py = tid >> 3, px = tid & 7;
 
-  for (int it = 0; it <= my_n; ++it) {
-    // (1) MMAs of tile it-1 are complete (frees halo stage (it+1)&1 and fills TMEM stage (it-1)&1)
-    if (it >= 1) mbar_wait(&mma_bar[(it - 1) & 1], ((it - 1) >> 1) & 1);
-    // (2) one thread starts the TMA load of tile it+1 (two stages; with one stage see (5))
+  for (int it = 0; it < my_n; ++it) {
+    // two stages: tile it+1 loads into the stage tile it-1 used (its MMAs completed in the last iteration)
     if (NB == 2 && tid == 0 && it + 1 < my_n) issue_halo(first + (it + 1) * stride, (it + 1) & 1);
-    // (3) MMAs of tile it as soon as its halo has landed
-    if (it < my_n) {
-      fence_before_sync();  // orders the previous iteration's tcgen05.ld (TMEM stage reuse)
-      __syncthreads();
-      if (tid == 0) {
-        mbar_wait(&ld_bar[NB == 2 ? (it & 1) : 0], NB == 2 ? ((it >> 1) & 1) : (it & 1));
-        fence_after_sync();
-        const uint32_t sh = s_halo0 + (uint32_t)(NB == 2 ? (it & 1) : 0) * STAGE;
-        const uint32_t tacc = tmem_base + (uint32_t)((it & 1) * N);
-        uint32_t accum = 0;
+    mbar_wait(&ld_bar[NB == 2 ? (it & 1) : 0], NB == 2 ? ((it >> 1) & 1) : (it & 1));
+    {
+      const uint32_t sh = s_halo0 + (uint32_t)(NB == 2 ? (it & 1) : 0) * STAGE;
+      wgmma_fence();
+      uint32_t accum = 0;
 #pragma unroll
-        for (int r = 0; r < KH; ++r)
+      for (int r = 0; r < KH; ++r)
 #pragma unroll
-          for (int s = 0; s < KW; ++s)
+        for (int s = 0; s < KW; ++s)
 #pragma unroll
-            for (int kk = 0; kk < C / 16; ++kk) {
-              const uint64_t da = make_smem_desc(sh + 2 * kk * SLAB + r * (HWD * 16) + s * 16, SLAB, HWD * 16, kNoSwizzle);
-              const uint64_t db = make_smem_desc(s_w + (r * KW + s) * (C * N * 2) + 2 * kk * (N * 16), N * 16, 128, kNoSwizzle);
-              mma_bf16_ss(tacc, da, db, idesc, accum);
-              accum = 1;
-            }
-        mma_commit(&mma_bar[it & 1]);
-      }
+          for (int kk = 0; kk < C / 16; ++kk) {
+            const uint64_t da = make_smem_desc(sh + 2 * kk * SLAB + r * (HWD * 16) + s * 16, SLAB, HWD * 16, kNoSwizzle);
+            const uint64_t db = make_smem_desc(s_w + (r * KW + s) * (C * N * 2) + 2 * kk * (N * 16), N * 16, 128, kNoSwizzle);
+            mma128<N, kT>(acc_t, da, 8 * HWD * 16, db, accum);
+            accum = 1;
+          }
+      wgmma_commit();
+      wgmma_wait<0>();
+      acc_fence(acc_t);
     }
-    // (4) epilogue of tile it-1 (same as conv_halo_kernel)
-    if (it >= 1) {
-      fence_after_sync();
+    // single halo stage: the MMAs of tile it have consumed it -> the next tile loads during this epilogue
+    if (NB == 1 && tid == 0 && it + 1 < my_n) issue_halo(first + (it + 1) * stride, 0);
+    {   // epilogue of tile it
       int b, oh0, ow0;
-      tile_coords(first + (it - 1) * stride, b, oh0, ow0);
-      const uint32_t taddr = tmem_base + ((uint32_t)(warp * 32) << 16) + (uint32_t)(((it - 1) & 1) * N);
+      tile_coords(first + it * stride, b, oh0, ow0);
       const size_t pix = ((size_t)b * a.H + oh0 + py) * a.W + ow0 + px;
-#pragma unroll 1
-      for (int col0 = 0; col0 < N; col0 += 32) {
-        uint32_t rr[32];
-        tmem_ld32(taddr + col0, rr);
-        tmem_ld_wait();
-        float acc[32];
 #pragma unroll
-        for (int j = 0; j < 32; ++j) acc[j] = __uint_as_float(rr[j]);
+      for (int col0 = 0; col0 < N; col0 += 32) {
+        float acc[32];
+        acc_row32(acc_t, col0, stage_buf, acc);
         if (MODE == 0 && a.stats != nullptr)
           halo_gn_stats_chunk(acc, lane, N / a.gn_groups, a.stats + (size_t)b * a.gn_groups * 2, col0);
         const size_t o = pix * N + col0;
@@ -961,15 +877,7 @@ conv_halo_tma_kernel(const HaloArgs a, const __grid_constant__ CUtensorMap tmap)
         }
       }
     }
-    // (5) single halo stage: tile it+1 may be loaded once the MMAs of tile it have consumed the stage
-    if (NB == 1 && tid == 0 && it + 1 < my_n) {
-      mbar_wait(&mma_bar[it & 1], (it >> 1) & 1);
-      issue_halo(first + (it + 1) * stride, 0);
-    }
   }
-  fence_before_sync();
-  __syncthreads();
-  if (warp == 0) tmem_dealloc(tmem_base, Cfg::TMEM_COLS);
 }
 
 template <int C, int N, int MODE>
@@ -977,8 +885,8 @@ __global__ void __launch_bounds__(128)
 conv_halo_sw_kernel(const HaloArgs a, const __grid_constant__ CUtensorMap tmap) {
   // 3x3 stride-1 pad-1.  The halo is staged as KW = 3 copies of the tile rows, copy kx pre-shifted by kx pixels, each
   // copy [HH rows][8 pixels][C channels] in the 64- / 128-byte-swizzle K-major layout (one TMA box per copy: rows of
-  // C*2 bytes instead of the 16-byte pieces of the no-swizzle slabs, whose rate -- not bytes -- bounded the halo kernels
-  // at ~2.1 TB/s).  A filter tap (r, s) is then copy s shifted by r whole swizzle atoms: aligned descriptors only.
+  // C*2 bytes instead of the 16-byte pieces of the no-swizzle slabs, whose rate -- not bytes -- bounds the slab-fed
+  // kernels).  A filter tap (r, s) is then copy s shifted by r whole swizzle atoms: aligned descriptors only.
   using Cfg = HaloCfg<C, N, 3, 3, 1>;
   constexpr int KH = 3, KW = 3, PAD = 1, HH = Cfg::HH;
   constexpr uint32_t RB = C * 2;                 // bytes per pixel row of the operand: 64 (SWIZZLE_64B) or 128
@@ -989,22 +897,18 @@ conv_halo_sw_kernel(const HaloArgs a, const __grid_constant__ CUtensorMap tmap) 
   constexpr int kSw = RB == 128 ? kSwizzle128B : kSwizzle64B;
   static_assert(RB == 64 || RB == 128, "conv_halo_sw: 32 or 64 channels");
   extern __shared__ __align__(16) uint8_t smem_raw[];
-  __shared__ __align__(8) uint64_t mma_bar[2];
   __shared__ __align__(8) uint64_t ld_bar[2];
-  __shared__ uint32_t tmem_slot;
+  __shared__ float stage_buf[kStageFloats];
   const uint32_t sbase = (smem_u32(smem_raw) + 1023u) & ~1023u;   // swizzle atoms: 1024-byte aligned
   const uint32_t s_w = sbase;
   const uint32_t s_halo0 = s_w + Cfg::W_BYTES;   // W_BYTES is a multiple of 128
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int tid = threadIdx.x, lane = tid & 31;
 
   if (tid == 0) {
-    mbar_init(&mma_bar[0], 1);
-    mbar_init(&mma_bar[1], 1);
     mbar_init(&ld_bar[0], 1);
     mbar_init(&ld_bar[1], 1);
     mbar_fence_init();
   }
-  if (warp == 0) tmem_alloc(&tmem_slot, Cfg::TMEM_COLS);
   {
     const uint4* src = reinterpret_cast<const uint4*>(a.wimg);
     for (int v = tid; v < Cfg::W_BYTES / 16; v += 128) cp_async16(s_w + (uint32_t)v * 16, src + v, true);
@@ -1033,61 +937,49 @@ conv_halo_sw_kernel(const HaloArgs a, const __grid_constant__ CUtensorMap tmap) 
   };
   const int first = blockIdx.x, stride = gridDim.x;
   const int my_n = first < a.ntiles ? (a.ntiles - first + stride - 1) / stride : 0;
+  __syncthreads();   // barriers initialised
   if (tid == 0 && my_n > 0) issue_halo(first, 0);
   cp_async_wait<0>();          // weights
-  fence_proxy_async_smem();    // cp.async (generic proxy) -> tcgen05 (async proxy)
-  fence_before_sync();
+  fence_proxy_async_smem();    // cp.async (generic proxy) -> wgmma (async proxy)
   __syncthreads();
-  fence_after_sync();
-  const uint32_t tmem_base = tmem_slot;
   // forward: fp16 input halo x fp16 weight image; dgrad: bf16 gradients x bf16 flipped / transposed image
-  constexpr uint32_t idesc = MODE == 0 ? make_idesc_f16(128, N, 0, 0, kFmtF16, kFmtF16) : make_idesc_bf16(128, N, 0, 0);
+  constexpr int kT = MODE == 0 ? kF16 : kBF16;
+  float acc_t[N];
   const int py = tid >> 3, px = tid & 7;
 
-  for (int it = 0; it <= my_n; ++it) {
-    // (1) MMAs of tile it-1 are complete (frees halo stage (it+1)&1 and fills TMEM stage (it-1)&1)
-    if (it >= 1) mbar_wait(&mma_bar[(it - 1) & 1], ((it - 1) >> 1) & 1);
-    // (2) one thread starts the TMA load of tile it+1 (two stages; with one stage see (5))
+  for (int it = 0; it < my_n; ++it) {
+    // two stages: tile it+1 loads into the stage tile it-1 used (its MMAs completed in the last iteration)
     if (NB == 2 && tid == 0 && it + 1 < my_n) issue_halo(first + (it + 1) * stride, (it + 1) & 1);
-    // (3) MMAs of tile it as soon as its halo has landed
-    if (it < my_n) {
-      fence_before_sync();  // orders the previous iteration's tcgen05.ld (TMEM stage reuse)
-      __syncthreads();
-      if (tid == 0) {
-        mbar_wait(&ld_bar[NB == 2 ? (it & 1) : 0], NB == 2 ? ((it >> 1) & 1) : (it & 1));
-        fence_after_sync();
-        const uint32_t sh = s_halo0 + (uint32_t)(NB == 2 ? (it & 1) : 0) * STAGE;
-        const uint32_t tacc = tmem_base + (uint32_t)((it & 1) * N);
-        uint32_t accum = 0;
+    mbar_wait(&ld_bar[NB == 2 ? (it & 1) : 0], NB == 2 ? ((it >> 1) & 1) : (it & 1));
+    {
+      const uint32_t sh = s_halo0 + (uint32_t)(NB == 2 ? (it & 1) : 0) * STAGE;
+      wgmma_fence();
+      uint32_t accum = 0;
 #pragma unroll
-        for (int r = 0; r < KH; ++r)
+      for (int r = 0; r < KH; ++r)
 #pragma unroll
-          for (int s = 0; s < KW; ++s)
+        for (int s = 0; s < KW; ++s)
 #pragma unroll
-            for (int kk = 0; kk < C / 16; ++kk) {
-              const uint64_t da = make_smem_desc(sh + s * COPY + r * ATOM + kk * 32, 16, ATOM, (Layout)kSw);
-              const uint64_t db = make_smem_desc(s_w + (r * KW + s) * (C * N * 2) + 2 * kk * (N * 16), N * 16, 128, kNoSwizzle);
-              mma_bf16_ss(tacc, da, db, idesc, accum);
-              accum = 1;
-            }
-        mma_commit(&mma_bar[it & 1]);
-      }
+          for (int kk = 0; kk < C / 16; ++kk) {
+            const uint64_t da = make_smem_desc(sh + s * COPY + r * ATOM + kk * 32, 16, ATOM, (Layout)kSw);
+            const uint64_t db = make_smem_desc(s_w + (r * KW + s) * (C * N * 2) + 2 * kk * (N * 16), N * 16, 128, kNoSwizzle);
+            mma128<N, kT>(acc_t, da, 8 * ATOM, db, accum);
+            accum = 1;
+          }
+      wgmma_commit();
+      wgmma_wait<0>();
+      acc_fence(acc_t);
     }
-    // (4) epilogue of tile it-1 (same as conv_halo_kernel)
-    if (it >= 1) {
-      fence_after_sync();
+    // single halo stage: the MMAs of tile it have consumed it -> the next tile loads during this epilogue
+    if (NB == 1 && tid == 0 && it + 1 < my_n) issue_halo(first + (it + 1) * stride, 0);
+    {   // epilogue of tile it
       int b, oh0, ow0;
-      tile_coords(first + (it - 1) * stride, b, oh0, ow0);
-      const uint32_t taddr = tmem_base + ((uint32_t)(warp * 32) << 16) + (uint32_t)(((it - 1) & 1) * N);
+      tile_coords(first + it * stride, b, oh0, ow0);
       const size_t pix = ((size_t)b * a.H + oh0 + py) * a.W + ow0 + px;
-#pragma unroll 1
-      for (int col0 = 0; col0 < N; col0 += 32) {
-        uint32_t rr[32];
-        tmem_ld32(taddr + col0, rr);
-        tmem_ld_wait();
-        float acc[32];
 #pragma unroll
-        for (int j = 0; j < 32; ++j) acc[j] = __uint_as_float(rr[j]);
+      for (int col0 = 0; col0 < N; col0 += 32) {
+        float acc[32];
+        acc_row32(acc_t, col0, stage_buf, acc);
         if (MODE == 0 && a.stats != nullptr)
           halo_gn_stats_chunk(acc, lane, N / a.gn_groups, a.stats + (size_t)b * a.gn_groups * 2, col0);
         const size_t o = pix * N + col0;
@@ -1120,31 +1012,21 @@ conv_halo_sw_kernel(const HaloArgs a, const __grid_constant__ CUtensorMap tmap) 
         }
       }
     }
-    // (5) single halo stage: tile it+1 may be loaded once the MMAs of tile it have consumed the stage
-    if (NB == 1 && tid == 0 && it + 1 < my_n) {
-      mbar_wait(&mma_bar[it & 1], (it >> 1) & 1);
-      issue_halo(first + (it + 1) * stride, 0);
-    }
   }
-  fence_before_sync();
-  __syncthreads();
-  if (warp == 0) tmem_dealloc(tmem_base, Cfg::TMEM_COLS);
 }
 
 
 // ---- warp-specialised variant ---------------------------------------------------------------------------------------
-// conv_halo_tma_kernel runs load -> MMA -> epilogue of consecutive tiles from ONE thread's program order: with a single
-// halo stage the TMA latency of tile it+1 (~1.5-2 us) is exposed after every tile, and only the second CTA of the SM
-// hides it (64-channel dgrad: 3.6 us per tile per CTA for 0.6 us of MMAs).  Here the three phases are separate warps
-// that meet only at mbarriers:
+// conv_halo_tma_kernel runs load -> MMA -> epilogue of consecutive tiles from one program order: with a single halo
+// stage the TMA latency of tile it+1 is exposed after every tile, and only a second CTA of the SM hides it.  Here the
+// loads run in their own warp and meet the consumers only at mbarriers:
 //   warp 4 (one lane)  producer: halo stage ring, NS deep (as many as fit next to the resident weights)
-//   warp 5 (one lane)  MMA issue: waits full[stage] + the accumulator's release, commits to empty[stage] and tfull[acc]
-//   warps 0-3          epilogue: TMEM -> registers, release the accumulator right after the last tcgen05.ld, then
-//                      GroupNorm sums / addend / pack / store while the next tile's MMAs already run
+//   warps 0-3          one warpgroup: waits full[stage], issues the tile's MMAs, releases the stage (empty[stage]) as
+//                      soon as they complete, then GroupNorm sums / addend / pack / store while the producer loads ahead
 // SW: stage the halo as KW pre-shifted copies of whole pixel rows in the swizzled K-major layout (conv_halo_sw_kernel)
 // instead of 16-byte channel slabs: aligned operand reads for the MMAs at KW times the TMA bytes
 template <int C, int N, int KH, int KW, int PAD, int MODE, int NS, bool SW = false>
-__global__ void __launch_bounds__(192)
+__global__ void __launch_bounds__(160)
 conv_halo_ws_kernel(const HaloArgs a, const __grid_constant__ CUtensorMap tmap) {
   using Cfg = HaloCfg<C, N, KH, KW, PAD>;
   constexpr int CJ = Cfg::CJ, HH = Cfg::HH, HWD = Cfg::HWD;
@@ -1154,8 +1036,8 @@ conv_halo_ws_kernel(const HaloArgs a, const __grid_constant__ CUtensorMap tmap) 
   constexpr int kSw = RB == 128 ? kSwizzle128B : kSwizzle64B;
   static_assert(!SW || RB == 64 || RB == 128, "swizzled halo copies: 32 or 64 channels");
   extern __shared__ __align__(16) uint8_t smem_raw[];
-  __shared__ __align__(8) uint64_t full_bar[NS], empty_bar[NS], tfull_bar[2], tempty_bar[2];
-  __shared__ uint32_t tmem_slot;
+  __shared__ __align__(8) uint64_t full_bar[NS], empty_bar[NS];
+  __shared__ float stage_buf[kStageFloats];
   const uint32_t sbase = (smem_u32(smem_raw) + 1023u) & ~1023u;   // swizzle atoms are 1024-byte aligned
   const uint32_t s_w = sbase;
   const uint32_t s_halo0 = s_w + Cfg::W_BYTES;
@@ -1163,22 +1045,16 @@ conv_halo_ws_kernel(const HaloArgs a, const __grid_constant__ CUtensorMap tmap) 
   if (tid == 0) {
 #pragma unroll
     for (int i = 0; i < NS; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 1); }
-    mbar_init(&tfull_bar[0], 1); mbar_init(&tfull_bar[1], 1);
-    mbar_init(&tempty_bar[0], 4); mbar_init(&tempty_bar[1], 4);   // one arrival per epilogue warp
     mbar_fence_init();
   }
-  if (warp == 0) tmem_alloc(&tmem_slot, Cfg::TMEM_COLS);
   {
     const uint4* src = reinterpret_cast<const uint4*>(a.wimg);
-    for (int v = tid; v < Cfg::W_BYTES / 16; v += 192) cp_async16(s_w + (uint32_t)v * 16, src + v, true);
+    for (int v = tid; v < Cfg::W_BYTES / 16; v += blockDim.x) cp_async16(s_w + (uint32_t)v * 16, src + v, true);
   }
   cp_async_commit();
   cp_async_wait<0>();
   fence_proxy_async_smem();
-  fence_before_sync();
   __syncthreads();
-  fence_after_sync();
-  const uint32_t tmem_base = tmem_slot;
   const int tiles_x = a.W / TW, tiles_per_img = tiles_x * (a.H / TH);
   const int first = blockIdx.x, stride = gridDim.x;
   const int my_n = first < a.ntiles ? (a.ntiles - first + stride - 1) / stride : 0;
@@ -1208,58 +1084,41 @@ conv_halo_ws_kernel(const HaloArgs a, const __grid_constant__ CUtensorMap tmap) 
       }
     }
     __syncwarp();
-  } else if (warp == 5) {
-    if (lane == 0) {
-      // forward: fp16 input halo x fp16 weight image; dgrad: bf16 gradients x bf16 flipped / transposed image
-      constexpr uint32_t idesc = MODE == 0 ? make_idesc_f16(128, N, 0, 0, kFmtF16, kFmtF16) : make_idesc_bf16(128, N, 0, 0);
-      for (int it = 0; it < my_n; ++it) {
-        const int st = it % NS, acc = it & 1;
-        if (it >= 2) mbar_wait(&tempty_bar[acc], ((it >> 1) - 1) & 1);
-        mbar_wait(&full_bar[st], (it / NS) & 1);
-        fence_after_sync();
-        const uint32_t sh = s_halo0 + (uint32_t)st * STAGE;
-        const uint32_t tacc = tmem_base + (uint32_t)(acc * N);
-        uint32_t accum = 0;
-#pragma unroll
-        for (int r = 0; r < KH; ++r)
-#pragma unroll
-          for (int s = 0; s < KW; ++s)
-#pragma unroll
-            for (int kk = 0; kk < C / 16; ++kk) {
-              const uint64_t da = SW ? make_smem_desc(sh + s * COPY + r * ATOM + kk * 32, 16, ATOM, (Layout)kSw)
-                                     : make_smem_desc(sh + 2 * kk * SLAB + r * (HWD * 16) + s * 16, SLAB, HWD * 16, kNoSwizzle);
-              const uint64_t db = make_smem_desc(s_w + (r * KW + s) * (C * N * 2) + 2 * kk * (N * 16), N * 16, 128, kNoSwizzle);
-              mma_bf16_ss(tacc, da, db, idesc, accum);
-              accum = 1;
-            }
-        mma_commit(&empty_bar[st]);    // the halo stage is free once these MMAs have read it
-        mma_commit(&tfull_bar[acc]);   // ... and the accumulator is complete
-      }
-    }
-    __syncwarp();
   } else {
+    // forward: fp16 input halo x fp16 weight image; dgrad: bf16 gradients x bf16 flipped / transposed image
+    constexpr int kT = MODE == 0 ? kF16 : kBF16;
     const int py = tid >> 3, px = tid & 7;
+    float acc_t[N];
     for (int it = 0; it < my_n; ++it) {
-      const int acc = it & 1;
+      const int st = it % NS;
       const int tile = first + it * stride;
       const int b = tile / tiles_per_img, r = tile - b * tiles_per_img;
       const int oh0 = (r / tiles_x) * TH, ow0 = (r % tiles_x) * TW;
-      mbar_wait(&tfull_bar[acc], (it >> 1) & 1);
-      fence_after_sync();
-      const uint32_t taddr = tmem_base + ((uint32_t)(warp * 32) << 16) + (uint32_t)(acc * N);
-      const size_t pix = ((size_t)b * a.H + oh0 + py) * a.W + ow0 + px;
-      uint32_t rr[N];
+      mbar_wait(&full_bar[st], (it / NS) & 1);
+      const uint32_t sh = s_halo0 + (uint32_t)st * STAGE;
+      wgmma_fence();
+      uint32_t accum = 0;
 #pragma unroll
-      for (int col0 = 0; col0 < N; col0 += 32) tmem_ld32(taddr + col0, *reinterpret_cast<uint32_t(*)[32]>(&rr[col0]));
-      tmem_ld_wait();
-      fence_before_sync();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tempty_bar[acc]);   // the MMA warp may overwrite this accumulator now
+      for (int r = 0; r < KH; ++r)
+#pragma unroll
+        for (int s = 0; s < KW; ++s)
+#pragma unroll
+          for (int kk = 0; kk < C / 16; ++kk) {
+            const uint64_t da = SW ? make_smem_desc(sh + s * COPY + r * ATOM + kk * 32, 16, ATOM, (Layout)kSw)
+                                   : make_smem_desc(sh + 2 * kk * SLAB + r * (HWD * 16) + s * 16, SLAB, HWD * 16, kNoSwizzle);
+            const uint64_t db = make_smem_desc(s_w + (r * KW + s) * (C * N * 2) + 2 * kk * (N * 16), N * 16, 128, kNoSwizzle);
+            mma128<N, kT>(acc_t, da, SW ? 8 * ATOM : 8 * HWD * 16, db, accum);
+            accum = 1;
+          }
+      wgmma_commit();
+      wgmma_wait<0>();
+      acc_fence(acc_t);
+      if (tid == 0) mbar_arrive(&empty_bar[st]);   // the halo stage is free: the producer may refill it
+      const size_t pix = ((size_t)b * a.H + oh0 + py) * a.W + ow0 + px;
 #pragma unroll
       for (int col0 = 0; col0 < N; col0 += 32) {
         float acc_[32];
-#pragma unroll
-        for (int j = 0; j < 32; ++j) acc_[j] = __uint_as_float(rr[col0 + j]);
+        acc_row32(acc_t, col0, stage_buf, acc_);
         if (MODE == 0 && a.stats != nullptr)
           halo_gn_stats_chunk(acc_, lane, N / a.gn_groups, a.stats + (size_t)b * a.gn_groups * 2, col0);
         const size_t o = pix * N + col0;
@@ -1293,9 +1152,6 @@ conv_halo_ws_kernel(const HaloArgs a, const __grid_constant__ CUtensorMap tmap) 
       }
     }
   }
-  fence_before_sync();
-  __syncthreads();
-  if (warp == 0) tmem_dealloc(tmem_base, Cfg::TMEM_COLS);
 }
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
@@ -1313,16 +1169,14 @@ static EncodeTiledFn halo_encode_fn() {
   return fn;
 }
 
-static int blocks_per_sm(const void* kern, size_t smem, int tmem_cols, int* cache) {
+static int blocks_per_sm(const void* kern, size_t smem, int* cache) {
   if (*cache > 0) return *cache;
   cudaFuncAttributes fa;
   if (cudaFuncGetAttributes(&fa, kern) != cudaSuccess) return 1;
   const int regs = fa.numRegs > 0 ? fa.numRegs : 128;
   int by_regs = 65536 / (((regs + 7) / 8 * 8) * 128);
   int by_smem = (int)((227 * 1024) / (smem + fa.sharedSizeBytes + 1024));
-  int by_tmem = 512 / tmem_cols;
   int n = by_regs < by_smem ? by_regs : by_smem;
-  if (by_tmem < n) n = by_tmem;
   if (n > 16) n = 16;
   if (n < 1) n = 1;
   *cache = n;
@@ -1336,7 +1190,7 @@ static int launch_halo(const HaloArgs& a, cudaStream_t st) {
   auto kern = conv_halo_kernel<C, N, KH, KW, PAD, MODE>;
   static int cache = 0;
   if (cache == 0) HB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  const int per_sm = blocks_per_sm((const void*)kern, smem, Cfg::TMEM_COLS, &cache);
+  const int per_sm = blocks_per_sm((const void*)kern, smem, &cache);
   int grid = kNumSMs * per_sm;
   if (grid > a.ntiles) grid = a.ntiles;
   kern<<<grid, 128, smem, st>>>(a);
@@ -1371,7 +1225,7 @@ static int launch_halo_tma(const HaloArgs& a, cudaStream_t st) {
   auto kern = conv_halo_tma_kernel<C, N, KH, KW, PAD, MODE>;
   static int cache = 0;
   if (cache == 0) HB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  const int per_sm = blocks_per_sm((const void*)kern, smem, Cfg::TMEM_COLS, &cache);
+  const int per_sm = blocks_per_sm((const void*)kern, smem, &cache);
   int grid = kNumSMs * per_sm;
   if (grid > a.ntiles) grid = a.ntiles;
   kern<<<grid, 128, smem, st>>>(a, tmap);
@@ -1410,20 +1264,18 @@ static int launch_halo_ws(const HaloArgs& a, cudaStream_t st) {
   static int grid_cache = 0;
   if (grid_cache == 0) {
     HB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    // resident CTAs per SM from the static limits (registers of 192 threads, shared memory, TMEM columns); the
-    // occupancy API reported 1 for these kernels on the B200 boxes (ncu: grid 148 where 3 CTAs per SM fit)
+    // resident CTAs per SM from the static limits (registers of 160 threads, shared memory)
     cudaFuncAttributes fa;
     HB_CUDA(cudaFuncGetAttributes(&fa, (const void*)kern));
     const int regs = fa.numRegs > 0 ? fa.numRegs : 128;
-    int per_sm = 65536 / (((regs + 7) / 8 * 8) * 192);
+    int per_sm = 65536 / (((regs + 7) / 8 * 8) * 160);
     const int by_smem = (int)((227 * 1024) / (smem + fa.sharedSizeBytes + 1024));
     if (by_smem < per_sm) per_sm = by_smem;
-    if (per_sm > 512 / Cfg::TMEM_COLS) per_sm = 512 / Cfg::TMEM_COLS;
     if (per_sm < 1) per_sm = 1;
     grid_cache = kNumSMs * per_sm;
   }
   const int grid = grid_cache < a.ntiles ? grid_cache : a.ntiles;
-  kern<<<grid, 192, smem, st>>>(a, tmap);
+  kern<<<grid, 160, smem, st>>>(a, tmap);
   HB_LAUNCH_OK();
   count_launch(1);
   return HB200_OK;
@@ -1455,7 +1307,7 @@ static int launch_halo_sw(const HaloArgs& a, cudaStream_t st) {
   auto kern = conv_halo_sw_kernel<C, N, MODE>;
   static int cache = 0;
   if (cache == 0) HB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  const int per_sm = blocks_per_sm((const void*)kern, smem, Cfg::TMEM_COLS, &cache);
+  const int per_sm = blocks_per_sm((const void*)kern, smem, &cache);
   int grid = kNumSMs * per_sm;
   if (grid > a.ntiles) grid = a.ntiles;
   kern<<<grid, 128, smem, st>>>(a, tmap);
@@ -1469,7 +1321,7 @@ static int launch_halo_wgrad(const HaloWgradArgs& a, cudaStream_t st) {
   constexpr int CJ = C / 8, HWD = TW + KW - 1, P = HWD * 16, RP = CJ * P;
   constexpr int MT = (KH * CJ + 15) / 16, RMAX = (MT * 16 + CJ - 1) / CJ, HROWS = TH - 1 + RMAX;
   constexpr int STAGE = (128 * N * 2 + HROWS * RP + 1023) / 1024 * 1024;
-  constexpr int NSW = (XMODE != 0 && C >= 64) ? 4 : 2;   // ring depth: must match the kernel
+  constexpr int NSW = halo_wgrad_stages(XMODE, C, STAGE);
   const size_t smem = NSW * (size_t)STAGE + 1024 + 64;
   EncodeTiledFn enc = halo_encode_fn();
   if (!enc) {
@@ -1513,15 +1365,24 @@ static int launch_halo_wgrad(const HaloWgradArgs& a, cudaStream_t st) {
   auto kern = conv_halo_wgrad_kernel<C, N, KH, KW, PAD, XMODE>;
   static int cache = 0;
   if (cache == 0) HB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  constexpr int raw = KW * MT * N;
-  constexpr int tcols = raw <= 32 ? 32 : raw <= 64 ? 64 : raw <= 128 ? 128 : raw <= 256 ? 256 : 512;
-  const int per_sm = blocks_per_sm((const void*)kern, smem, tcols, &cache);
-  int grid = kNumSMs * per_sm;
+  // accumulator groups (the kernel's APC): one grid row each, every row walks all tiles
+  constexpr int nacc = KW * MT, ngrp = nacc * N <= 128 ? 1 : nacc / (128 / N);
+  const int per_sm = blocks_per_sm((const void*)kern, smem, &cache);
+  int grid = kNumSMs * per_sm / ngrp;
+  if (grid < 1) grid = 1;
   if (grid > a.ntiles) grid = a.ntiles;
-  kern<<<grid, 128, smem, st>>>(a, tmap, tmap_x);
+  // one partial per worker column, summed in worker order into the caller's accumulator (deterministic)
+  const long long count = (long long)KH * KW * C * N;
+  float* parts = nullptr;
+  int* tickets = nullptr;
+  int rc = stream_workspace(st, (size_t)(grid + (grid < kReduceChunks ? grid : kReduceChunks)) * count, 0, &parts, &tickets);
+  if (rc) return rc;
+  HaloWgradArgs ap = a;
+  ap.dw = parts;
+  kern<<<dim3(grid, ngrp), 128, smem, st>>>(ap, tmap, tmap_x);
   HB_LAUNCH_OK();
   count_launch(1);
-  return HB200_OK;
+  return reduce_partials(parts, grid, count, count, a.dw, parts + (size_t)grid * count, st);
 }
 
 template <int NS, int IMG>
@@ -1556,14 +1417,23 @@ static int launch_halo_wgrad_small(const HaloWgradSmallArgs& a, cudaStream_t st)
     HB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     attr = true;
   }
-  const int slices = (a.Ci / 32) * (a.Co / NS);
-  int workers = kNumSMs / slices;            // one CTA per SM (3 x NS accumulator columns need most of TMEM)
+  const int slices = (a.Ci / 32) * (a.Co / NS) * 3;   // channel slices x the 3 horizontal taps (one accumulator each)
+  int workers = 2 * kNumSMs / slices;
   if (workers < 1) workers = 1;
   if (workers > a.ntiles) workers = a.ntiles;
-  kern<<<dim3(workers, slices), 128, smem, st>>>(a, tmap);
+  // one partial per worker, summed in worker order into the caller's accumulator (deterministic)
+  const long long count = 9LL * a.Ci * a.Co;
+  float* parts = nullptr;
+  int* tickets = nullptr;
+  int rc = stream_workspace(st, (size_t)(workers + (workers < kReduceChunks ? workers : kReduceChunks)) * count, 0, &parts,
+                            &tickets);
+  if (rc) return rc;
+  HaloWgradSmallArgs ap = a;
+  ap.dw = parts;
+  kern<<<dim3(workers, slices), 128, smem, st>>>(ap, tmap);
   HB_LAUNCH_OK();
   count_launch(1);
-  return HB200_OK;
+  return reduce_partials(parts, workers, count, count, a.dw, parts + (size_t)workers * count, st);
 }
 }  // namespace hb200
 
@@ -1571,7 +1441,6 @@ using namespace hb200;
 
 // halo loads by TMA (default) or by the cp.async gather kernel (HB200_NO_HALO_TMA=1, or hb200_set_halo_tma(0) from tests)
 static int g_halo_tma = getenv("HB200_NO_HALO_TMA") == nullptr ? 1 : 0;
-// 4096 frames: 32-channel layers 172 -> 159 us, 64-channel 169 -> 133 us, stem 671 -> 650 us with the TMA box
 static int g_wgrad_xtma = getenv("HB200_WGRAD_XTMA") ? atoi(getenv("HB200_WGRAD_XTMA")) : 1;
 extern "C" int hb200_set_halo_tma(int enable) {
   g_halo_tma = enable;   // 0 cp.async gather, 1 best per layer (default), 2 swizzled rows, 3 warp-specialised slabs, 4 both, 5 plain TMA slabs
@@ -1627,19 +1496,17 @@ extern "C" int hb200_conv_halo(const hb200_bf16* x, const hb200_bf16* wimg, hb20
   a.B = batch; a.H = h; a.W = w; a.gn_groups = gn_groups > 0 ? gn_groups : 1;
   a.ntiles = batch * (h / TH) * (w / TW);
   cudaStream_t st = (cudaStream_t)stream;
-  // TMA-fed halo (conv_halo_tma_kernel) for every halo layer: measured 17-18 % faster than the cp.async gather on
-  // B200 for the 32-channel layers and the stem (0.219 -> 0.183 ms, 0.711 -> 0.581 ms); HB200_NO_HALO_TMA=1 disables
+  // TMA-fed halo for every halo layer (no per-thread address / predicate work); HB200_NO_HALO_TMA=1 disables
   const bool use_tma = g_halo_tma != 0;
-  // Loader per layer (hb200_set_halo_tma): 1 = the measured best of the variants below (tools/halo_bench.py, 4096 frames):
-  //   64 channels: warp-specialised + swizzled pixel-row copies  fwd 126 -> 93 us, dgrad 99 -> 88 us
-  //   32 channels: warp-specialised + swizzled copies  fwd 176 -> 140 us, dgrad 177 -> 143 us
+  // Loader per layer (hb200_set_halo_tma): 1 = the default per layer below (compare with tools/halo_bench.py):
+  //   64 / 32 channels: warp-specialised + swizzled pixel-row copies; the stem: warp-specialised slabs
   // 2 / 3 / 4 / 5 force swizzled copies / warp-specialised slabs / warp-specialised swizzled / plain slabs everywhere.
   if (g_halo_tma == 1 && k == 3 && c == 64)
     return mode == 0 ? launch_halo_ws<64, 64, 3, 3, 1, 0, 2, true>(a, st) : launch_halo_ws<64, 64, 3, 3, 1, 1, 2, true>(a, st);
-  if (g_halo_tma == 1 && k == 3 && c == 32)   // fwd 176 -> 140 us, dgrad 146 -> 143 us (two CTAs per SM, 3 stages each)
+  if (g_halo_tma == 1 && k == 3 && c == 32)   // 3 stages each: several CTAs per SM
     return mode == 0 ? launch_halo_ws<32, 32, 3, 3, 1, 0, 3, true>(a, st) : launch_halo_ws<32, 32, 3, 3, 1, 1, 3, true>(a, st);
-  if (g_halo_tma == 1 && k == 4 && mode == 0) return launch_halo_ws<16, 32, 4, 4, 2, 0, 6>(a, st);   // stem 564 -> 524 us
-  if (g_halo_tma == 6 && k == 3 && c == 32)   // experiment: 2 stages, three CTAs per SM (150 / 150 us: worse)
+  if (g_halo_tma == 1 && k == 4 && mode == 0) return launch_halo_ws<16, 32, 4, 4, 2, 0, 6>(a, st);
+  if (g_halo_tma == 6 && k == 3 && c == 32)   // experiment: 2 stages, more CTAs per SM
     return mode == 0 ? launch_halo_ws<32, 32, 3, 3, 1, 0, 2, true>(a, st) : launch_halo_ws<32, 32, 3, 3, 1, 1, 2, true>(a, st);
   if (g_halo_tma == 4 && k == 3 && c == 32)
     return mode == 0 ? launch_halo_ws<32, 32, 3, 3, 1, 0, 3, true>(a, st) : launch_halo_ws<32, 32, 3, 3, 1, 1, 3, true>(a, st);
@@ -1648,7 +1515,7 @@ extern "C" int hb200_conv_halo(const hb200_bf16* x, const hb200_bf16* wimg, hb20
   if (g_halo_tma == 3 && k == 3 && c == 32)
     return mode == 0 ? launch_halo_ws<32, 32, 3, 3, 1, 0, 4>(a, st) : launch_halo_ws<32, 32, 3, 3, 1, 1, 4>(a, st);
   if (g_halo_tma == 3 && k == 3 && c == 64)
-    return mode == 0 ? launch_halo_ws<64, 64, 3, 3, 1, 0, 6>(a, st) : launch_halo_ws<64, 64, 3, 3, 1, 1, 6>(a, st);
+    return mode == 0 ? launch_halo_ws<64, 64, 3, 3, 1, 0, 5>(a, st) : launch_halo_ws<64, 64, 3, 3, 1, 1, 5>(a, st);
   if (g_halo_tma == 3 && k == 4 && mode == 0) return launch_halo_ws<16, 32, 4, 4, 2, 0, 6>(a, st);
   if (g_halo_tma == 2 && k == 3 && c == 32)
     return mode == 0 ? launch_halo_sw<32, 32, 0>(a, st) : launch_halo_sw<32, 32, 1>(a, st);
@@ -1657,8 +1524,8 @@ extern "C" int hb200_conv_halo(const hb200_bf16* x, const hb200_bf16* wimg, hb20
   if (use_tma && k == 3 && c == 32)
     return mode == 0 ? launch_halo_tma<32, 32, 3, 3, 1, 0>(a, st) : launch_halo_tma<32, 32, 3, 3, 1, 1>(a, st);
   if (use_tma && k == 4 && mode == 0) return launch_halo_tma<16, 32, 4, 4, 2, 0>(a, st);
-  // 64-channel layers: single halo stage (72 KB of resident weights), two CTAs per SM: 0.156 -> 0.146 ms forward,
-  // 0.128 -> 0.101 ms dgrad per layer against the cp.async gather (its 1440 copies per tile = 2880 LSU cycles)
+  // 64-channel layers: single halo stage (72 KB of resident weights), the load replaces the cp.async gather's 1440
+  // copies per tile
   if (use_tma && k == 3 && c == 64)
     return mode == 0 ? launch_halo_tma<64, 64, 3, 3, 1, 0>(a, st) : launch_halo_tma<64, 64, 3, 3, 1, 1>(a, st);
   if (k == 3 && c == 32) return mode == 0 ? launch_halo<32, 32, 3, 3, 1, 0>(a, st) : launch_halo<32, 32, 3, 3, 1, 1>(a, st);

@@ -11,20 +11,20 @@
 // (dims (dx,c) | bx | dy | by | b): no space-to-depth copy, no im2col, padding = out-of-range zero fill.
 // Both branches share the halo tile and the accumulator: output columns [0,NA) | [NA,NA+NB).
 //
-// The gather kernel (conv_igemm) spent 257 + 188 us (forward) and 602 + 286 us (dgrad) on these two convolutions of
-// layer2.0 at 4096 frames -- 8192 / 32768 CTAs with 1-5 K chunks each, fixed per-CTA costs dominating.
+// On the gather kernel (conv_igemm) these two convolutions of layer2.0 are 8192 / 32768 CTAs with 1-5 K chunks each at
+// 4096 frames: fixed per-CTA costs dominate.
 #include <cuda.h>
 #include <stdlib.h>
 
 #include "common.cuh"
-#include "umma.cuh"
+#include "wgmma.cuh"
 
 namespace hb200 {
 void count_launch(int n);
-using namespace umma;
+using namespace wg;
 
 namespace {
-constexpr int S2_TH = 16, S2_TW = 8;  // tile: 16 x 8 output pixels (forward) / 2x2 input blocks (dgrad) = UMMA M
+constexpr int S2_TH = 16, S2_TW = 8;  // tile: 16 x 8 output pixels (forward) / 2x2 input blocks (dgrad) = MMA M
 
 __device__ __forceinline__ float s2_warp_reduce16(float (&v)[16], int lane) {
   float a[8], b[4], c[2];
@@ -127,21 +127,17 @@ __global__ void __launch_bounds__(128) conv_s2_fwd_kernel(const S2Args a, const 
   constexpr int N = NA + NB, CJ = 4 * C / 8, CB = C / 8, HH = S2_TH + 1, HWD = S2_TW + 1;
   constexpr uint32_t SLAB = (uint32_t)((HH * HWD * 16 + 127) / 128 * 128);
   constexpr uint32_t W_BYTES = 9 * C * N * 2;
-  static_assert(N % 32 == 0 && NA % 32 == 0 && C % 16 == 0 && 2 * N <= 512, "conv_s2: unsupported channel counts");
+  static_assert(N % 32 == 0 && NA % 32 == 0 && C % 16 == 0 && N <= 128, "conv_s2: unsupported channel counts");
   extern __shared__ __align__(16) uint8_t smem_raw[];
-  __shared__ __align__(8) uint64_t mma_bar[2];
   __shared__ __align__(8) uint64_t ld_bar;
-  __shared__ uint32_t tmem_slot;
+  __shared__ float stage_buf[kStageFloats];
   const uint32_t sbase = (smem_u32(smem_raw) + 127u) & ~127u;
   const uint32_t s_w = sbase, s_halo = s_w + W_BYTES;
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int tid = threadIdx.x, lane = tid & 31;
   if (tid == 0) {
-    mbar_init(&mma_bar[0], 1);
-    mbar_init(&mma_bar[1], 1);
     mbar_init(&ld_bar, 1);
     mbar_fence_init();
   }
-  if (warp == 0) tmem_alloc(&tmem_slot, 2 * N);
   {
     const uint4* src = reinterpret_cast<const uint4*>(a.wimg);
     for (int v = tid; v < (int)(W_BYTES / 16); v += 128) cp_async16(s_w + (uint32_t)v * 16, src + v, true);
@@ -165,87 +161,65 @@ __global__ void __launch_bounds__(128) conv_s2_fwd_kernel(const S2Args a, const 
   };
   const int first = blockIdx.x, stride = gridDim.x;
   const int my_n = first < a.ntiles ? (a.ntiles - first + stride - 1) / stride : 0;
+  __syncthreads();   // barrier initialised
   if (tid == 0 && my_n > 0) issue_halo(first);
   cp_async_wait<0>();
   fence_proxy_async_smem();
-  fence_before_sync();
   __syncthreads();
-  fence_after_sync();
-  const uint32_t tmem_base = tmem_slot;
-  constexpr uint32_t idesc = make_idesc_f16(128, N, 0, 0, kFmtF16, kFmtF16);
   const int py = tid >> 3, px = tid & 7;
+  float acc_t[N];
 
-  for (int it = 0; it <= my_n; ++it) {
-    if (it >= 1) mbar_wait(&mma_bar[(it - 1) & 1], ((it - 1) >> 1) & 1);
-    if (it < my_n) {
-      fence_before_sync();  // orders the previous iteration's tcgen05.ld (TMEM stage reuse)
-      __syncthreads();
-      if (tid == 0) {
-        mbar_wait(&ld_bar, it & 1);
-        fence_after_sync();
-        const uint32_t tacc = tmem_base + (uint32_t)((it & 1) * N);
-        uint32_t accum = 0;
+  for (int it = 0; it < my_n; ++it) {
+    mbar_wait(&ld_bar, it & 1);
+    wgmma_fence();
+    uint32_t accum = 0;
 #pragma unroll
-        for (int r = 0; r < 3; ++r)
+    for (int r = 0; r < 3; ++r)
 #pragma unroll
-          for (int s = 0; s < 3; ++s)
+      for (int s = 0; s < 3; ++s)
 #pragma unroll
-            for (int kk = 0; kk < C / 16; ++kk) {
-              const int slab = (s2_d(r) * 2 + s2_d(s)) * CB + 2 * kk;
-              const uint64_t da = make_smem_desc(s_halo + slab * SLAB + s2_k(r) * (HWD * 16) + s2_k(s) * 16, SLAB,
-                                                 HWD * 16, kNoSwizzle);
-              const uint64_t db = make_smem_desc(s_w + (r * 3 + s) * (C * N * 2) + 2 * kk * (N * 16), N * 16, 128,
-                                                 kNoSwizzle);
-              mma_bf16_ss(tacc, da, db, idesc, accum);
-              accum = 1;
-            }
-        mma_commit(&mma_bar[it & 1]);
-      }
-    }
-    if (it >= 1) {   // epilogue of tile it-1
-      fence_after_sync();
-      int b, oh0, ow0;
-      tile_coords(first + (it - 1) * stride, b, oh0, ow0);
-      const uint32_t taddr = tmem_base + ((uint32_t)(warp * 32) << 16) + (uint32_t)(((it - 1) & 1) * N);
-      const size_t pix = ((size_t)b * a.Ho + oh0 + py) * a.Wo + ow0 + px;
-#pragma unroll 1
-      for (int col0 = 0; col0 < N; col0 += 32) {
-        uint32_t rr[32];
-        tmem_ld32(taddr + col0, rr);
-        tmem_ld_wait();
-        float acc[32];
-#pragma unroll
-        for (int j = 0; j < 32; ++j) acc[j] = __uint_as_float(rr[j]);
-        const bool second = col0 >= NA;
-        double* stats = second ? a.stats_b : a.stats_a;
-        if (stats != nullptr) {
-          const int groups = second ? a.groups_b : a.groups_a;
-          s2_gn_stats_chunk(acc, lane, (second ? NB : NA) / groups, stats + (size_t)b * groups * 2,
-                            col0 - (second ? NA : 0));
+        for (int kk = 0; kk < C / 16; ++kk) {
+          const int slab = (s2_d(r) * 2 + s2_d(s)) * CB + 2 * kk;
+          const uint64_t da = make_smem_desc(s_halo + slab * SLAB + s2_k(r) * (HWD * 16) + s2_k(s) * 16, SLAB,
+                                             HWD * 16, kNoSwizzle);
+          const uint64_t db = make_smem_desc(s_w + (r * 3 + s) * (C * N * 2) + 2 * kk * (N * 16), N * 16, 128,
+                                             kNoSwizzle);
+          mma128<N, kF16>(acc_t, da, 8 * HWD * 16, db, accum);
+          accum = 1;
         }
-        __half* out = second ? reinterpret_cast<__half*>(a.yb) + pix * NB + (col0 - NA)
-                             : reinterpret_cast<__half*>(a.ya) + pix * NA + col0;
-        uint4* dst = reinterpret_cast<uint4*>(out);
+    wgmma_commit();
+    wgmma_wait<0>();
+    acc_fence(acc_t);
+    // single halo stage: the MMAs of tile it have consumed it -> tile it+1 loads while this tile's epilogue runs
+    if (tid == 0 && it + 1 < my_n) issue_halo(first + (it + 1) * stride);
+    int b, oh0, ow0;
+    tile_coords(first + it * stride, b, oh0, ow0);
+    const size_t pix = ((size_t)b * a.Ho + oh0 + py) * a.Wo + ow0 + px;
 #pragma unroll
-        for (int v = 0; v < 4; ++v) {
-          uint4 u;
-          u.x = pack_f16x2(acc[v * 8 + 0], acc[v * 8 + 1]);
-          u.y = pack_f16x2(acc[v * 8 + 2], acc[v * 8 + 3]);
-          u.z = pack_f16x2(acc[v * 8 + 4], acc[v * 8 + 5]);
-          u.w = pack_f16x2(acc[v * 8 + 6], acc[v * 8 + 7]);
-          dst[v] = u;
-        }
+    for (int col0 = 0; col0 < N; col0 += 32) {
+      float acc[32];
+      acc_row32(acc_t, col0, stage_buf, acc);
+      const bool second = col0 >= NA;
+      double* stats = second ? a.stats_b : a.stats_a;
+      if (stats != nullptr) {
+        const int groups = second ? a.groups_b : a.groups_a;
+        s2_gn_stats_chunk(acc, lane, (second ? NB : NA) / groups, stats + (size_t)b * groups * 2,
+                          col0 - (second ? NA : 0));
       }
-    }
-    // single halo stage: tile it+1 is loaded once the MMAs of tile it have consumed it (the other CTA of the SM covers)
-    if (tid == 0 && it + 1 < my_n) {
-      mbar_wait(&mma_bar[it & 1], (it >> 1) & 1);
-      issue_halo(first + (it + 1) * stride);
+      __half* out = second ? reinterpret_cast<__half*>(a.yb) + pix * NB + (col0 - NA)
+                           : reinterpret_cast<__half*>(a.ya) + pix * NA + col0;
+      uint4* dst = reinterpret_cast<uint4*>(out);
+#pragma unroll
+      for (int v = 0; v < 4; ++v) {
+        uint4 u;
+        u.x = pack_f16x2(acc[v * 8 + 0], acc[v * 8 + 1]);
+        u.y = pack_f16x2(acc[v * 8 + 2], acc[v * 8 + 3]);
+        u.z = pack_f16x2(acc[v * 8 + 4], acc[v * 8 + 5]);
+        u.w = pack_f16x2(acc[v * 8 + 6], acc[v * 8 + 7]);
+        dst[v] = u;
+      }
     }
   }
-  fence_before_sync();
-  __syncthreads();
-  if (warp == 0) tmem_dealloc(tmem_base, 2 * N);
 }
 
 // ---- data gradient ----------------------------------------------------------------------------------------------------
@@ -259,21 +233,17 @@ __global__ void __launch_bounds__(128) conv_s2_dgrad_kernel(const S2Args a, cons
   constexpr int N = NA + NB, CJ = N / 8, CJA = NA / 8, HH = S2_TH + 1, HWD = S2_TW + 1, NOUT = 4 * C;
   constexpr uint32_t SLAB = (uint32_t)((HH * HWD * 16 + 127) / 128 * 128);
   constexpr uint32_t W_BYTES = 9 * C * N * 2;
-  static_assert(C % 16 == 0 && C >= 16 && N % 16 == 0 && 2 * NOUT <= 512, "conv_s2 dgrad: unsupported channel counts");
+  static_assert(C % 32 == 0 && C >= 32 && N % 16 == 0 && NOUT <= 128, "conv_s2 dgrad: unsupported channel counts");
   extern __shared__ __align__(16) uint8_t smem_raw[];
-  __shared__ __align__(8) uint64_t mma_bar[2];
   __shared__ __align__(8) uint64_t ld_bar;
-  __shared__ uint32_t tmem_slot;
+  __shared__ float stage_buf[kStageFloats];
   const uint32_t sbase = (smem_u32(smem_raw) + 127u) & ~127u;
   const uint32_t s_w = sbase, s_halo = s_w + W_BYTES;
-  const int tid = threadIdx.x, warp = tid >> 5;
+  const int tid = threadIdx.x;
   if (tid == 0) {
-    mbar_init(&mma_bar[0], 1);
-    mbar_init(&mma_bar[1], 1);
     mbar_init(&ld_bar, 1);
     mbar_fence_init();
   }
-  if (warp == 0) tmem_alloc(&tmem_slot, 2 * NOUT);
   {
     const uint4* src = reinterpret_cast<const uint4*>(a.wimg);
     for (int v = tid; v < (int)(W_BYTES / 16); v += 128) cp_async16(s_w + (uint32_t)v * 16, src + v, true);
@@ -300,144 +270,118 @@ __global__ void __launch_bounds__(128) conv_s2_dgrad_kernel(const S2Args a, cons
   };
   const int first = blockIdx.x, stride = gridDim.x;
   const int my_n = first < a.ntiles ? (a.ntiles - first + stride - 1) / stride : 0;
+  __syncthreads();   // barrier initialised
   if (tid == 0 && my_n > 0) issue_halo(first);
   cp_async_wait<0>();
   fence_proxy_async_smem();
-  fence_before_sync();
   __syncthreads();
-  fence_after_sync();
-  const uint32_t tmem_base = tmem_slot;
-  constexpr uint32_t idesc = make_idesc_bf16(128, C, 0, 0);
   const int py = tid >> 3, px = tid & 7;
   const int H = 2 * a.Ho, W = 2 * a.Wo;
+  float acc_q[4][C];   // one accumulator per output sub-pixel (dy, dx)
 
-  for (int it = 0; it <= my_n; ++it) {
-    if (it >= 1) mbar_wait(&mma_bar[(it - 1) & 1], ((it - 1) >> 1) & 1);
-    if (it < my_n) {
-      fence_before_sync();
-      __syncthreads();
-      if (tid == 0) {
-        mbar_wait(&ld_bar, it & 1);
-        fence_after_sync();
-        const uint32_t tacc = tmem_base + (uint32_t)((it & 1) * NOUT);
+  for (int it = 0; it < my_n; ++it) {
+    mbar_wait(&ld_bar, it & 1);
+    wgmma_fence();
 #pragma unroll
-        for (int dy = 0; dy < 2; ++dy)
+    for (int dy = 0; dy < 2; ++dy)
 #pragma unroll
-          for (int dx = 0; dx < 2; ++dx) {
-            uint32_t accum = 0;
+      for (int dx = 0; dx < 2; ++dx) {
+        uint32_t accum = 0;
 #pragma unroll
-            for (int r = 0; r < 3; ++r) {
-              if (((dy + 1 - r) & 1) != 0) continue;
+        for (int r = 0; r < 3; ++r) {
+          if (((dy + 1 - r) & 1) != 0) continue;
 #pragma unroll
-              for (int s = 0; s < 3; ++s) {
-                if (((dx + 1 - s) & 1) != 0) continue;
-                const int ky = (dy + 1 - r) / 2, kx = (dx + 1 - s) / 2;   // output pixel = block + (ky, kx): 0 or 1
-                const int tap = (2 - r) * 3 + (2 - s);                     // flipped storage of the mode-1 image
+          for (int s = 0; s < 3; ++s) {
+            if (((dx + 1 - s) & 1) != 0) continue;
+            const int ky = (dy + 1 - r) / 2, kx = (dx + 1 - s) / 2;   // output pixel = block + (ky, kx): 0 or 1
+            const int tap = (2 - r) * 3 + (2 - s);                     // flipped storage of the mode-1 image
 #pragma unroll
-                for (int kk = 0; kk < N / 16; ++kk) {
-                  const uint64_t da = make_smem_desc(s_halo + 2 * kk * SLAB + ky * (HWD * 16) + kx * 16, SLAB, HWD * 16,
-                                                     kNoSwizzle);
-                  const uint64_t db = make_smem_desc(s_w + tap * (C * N * 2) + 2 * kk * (C * 16), C * 16, 128,
-                                                     kNoSwizzle);
-                  mma_bf16_ss(tacc + (uint32_t)((dy * 2 + dx) * C), da, db, idesc, accum);
-                  accum = 1;
-                }
-              }
+            for (int kk = 0; kk < N / 16; ++kk) {
+              const uint64_t da = make_smem_desc(s_halo + 2 * kk * SLAB + ky * (HWD * 16) + kx * 16, SLAB, HWD * 16,
+                                                 kNoSwizzle);
+              const uint64_t db = make_smem_desc(s_w + tap * (C * N * 2) + 2 * kk * (C * 16), C * 16, 128,
+                                                 kNoSwizzle);
+              mma128<C, kBF16>(acc_q[dy * 2 + dx], da, 8 * HWD * 16, db, accum);
+              accum = 1;
             }
           }
-        mma_commit(&mma_bar[it & 1]);
-      }
-    }
-    if (it >= 1) {
-      fence_after_sync();
-      int b, oh0, ow0;
-      tile_coords(first + (it - 1) * stride, b, oh0, ow0);
-      const uint32_t taddr = tmem_base + ((uint32_t)(warp * 32) << 16) + (uint32_t)(((it - 1) & 1) * NOUT);
-#pragma unroll 1
-      for (int col0 = 0; col0 < NOUT; col0 += 32) {
-        uint32_t rr[32];
-        tmem_ld32(taddr + col0, rr);
-        tmem_ld_wait();
-        float acc[32];
-#pragma unroll
-        for (int j = 0; j < 32; ++j) acc[j] = __uint_as_float(rr[j]);
-        const int q = col0 / C, c0 = col0 - q * C;   // sub-pixel (dy,dx) = (q >> 1, q & 1), channel offset
-        const size_t o = ((((size_t)b * H + 2 * (oh0 + py) + (q >> 1)) * W) + 2 * (ow0 + px) + (q & 1)) * C + c0;
-        if (a.addend != nullptr) {
-          const uint4* ad = reinterpret_cast<const uint4*>(reinterpret_cast<const __nv_bfloat16*>(a.addend) + o);
-#pragma unroll
-          for (int v = 0; v < 4; ++v) {
-            float f[8];
-            unpack8(ad[v], f);
-#pragma unroll
-            for (int e = 0; e < 8; ++e) acc[v * 8 + e] += f[e];
-          }
         }
-        uint4* dst = reinterpret_cast<uint4*>(reinterpret_cast<__nv_bfloat16*>(a.ya) + o);
+      }
+    wgmma_commit();
+    wgmma_wait<0>();
+#pragma unroll
+    for (int q = 0; q < 4; ++q) acc_fence(acc_q[q]);
+    if (tid == 0 && it + 1 < my_n) issue_halo(first + (it + 1) * stride);
+    int b, oh0, ow0;
+    tile_coords(first + it * stride, b, oh0, ow0);
+#pragma unroll
+    for (int col0 = 0; col0 < NOUT; col0 += 32) {
+      const int q = col0 / C, c0 = col0 - q * C;   // sub-pixel (dy,dx) = (q >> 1, q & 1), channel offset
+      float acc[32];
+      acc_row32(acc_q[q], c0, stage_buf, acc);
+      const size_t o = ((((size_t)b * H + 2 * (oh0 + py) + (q >> 1)) * W) + 2 * (ow0 + px) + (q & 1)) * C + c0;
+      if (a.addend != nullptr) {
+        const uint4* ad = reinterpret_cast<const uint4*>(reinterpret_cast<const __nv_bfloat16*>(a.addend) + o);
 #pragma unroll
         for (int v = 0; v < 4; ++v) {
-          uint4 u;
-          u.x = pack_bf16x2(acc[v * 8 + 0], acc[v * 8 + 1]);
-          u.y = pack_bf16x2(acc[v * 8 + 2], acc[v * 8 + 3]);
-          u.z = pack_bf16x2(acc[v * 8 + 4], acc[v * 8 + 5]);
-          u.w = pack_bf16x2(acc[v * 8 + 6], acc[v * 8 + 7]);
-          dst[v] = u;
+          float f[8];
+          unpack8(ad[v], f);
+#pragma unroll
+          for (int e = 0; e < 8; ++e) acc[v * 8 + e] += f[e];
         }
       }
-    }
-    if (tid == 0 && it + 1 < my_n) {
-      mbar_wait(&mma_bar[it & 1], (it >> 1) & 1);
-      issue_halo(first + (it + 1) * stride);
+      uint4* dst = reinterpret_cast<uint4*>(reinterpret_cast<__nv_bfloat16*>(a.ya) + o);
+#pragma unroll
+      for (int v = 0; v < 4; ++v) {
+        uint4 u;
+        u.x = pack_bf16x2(acc[v * 8 + 0], acc[v * 8 + 1]);
+        u.y = pack_bf16x2(acc[v * 8 + 2], acc[v * 8 + 3]);
+        u.z = pack_bf16x2(acc[v * 8 + 4], acc[v * 8 + 5]);
+        u.w = pack_bf16x2(acc[v * 8 + 6], acc[v * 8 + 7]);
+        dst[v] = u;
+      }
     }
   }
-  fence_before_sync();
-  __syncthreads();
-  if (warp == 0) tmem_dealloc(tmem_base, 2 * NOUT);
 }
 
 // ---- warp-specialised variant with swizzled pixel-row copies (default) ------------------------------------------------
-// The kernels above feed the tensor core from 16-byte TMA pieces (8-channel slabs): every slab-fed kernel of this library
-// tops out near 12 B / clk / SM of TMA traffic (~3.4 TB/s).  Here a stage holds FOUR copies of the tile rows, each
-// [17 rows][8 pixels][128 B] in the 128-byte-swizzle K-major layout, one TMA box each (128-byte rows: 8x fewer pieces):
+// The kernels above feed the tensor core from 16-byte TMA pieces (8-channel slabs).  Here a stage holds FOUR copies of
+// the tile rows, each [17 rows][8 pixels][128 B] in the 128-byte-swizzle K-major layout, one TMA box each (128-byte rows:
+// 8x fewer pieces):
 //   forward: copy (dy, kx) = sub-row dy of the space-to-depth view, pre-shifted by kx block columns; a filter tap (r, s) reads
 //            copy (dy(r), kx(s)) shifted by ky(r) whole atoms, K offset dx(s) * 64 B inside the 128-byte (dx, c) row
 //   dgrad:   copy (t, kx) = tensor t of (dya | dyb) pre-shifted by kx; K block kk of the 128 reduction channels reads
 //            tensor kk / 4 at K offset (kk % 4) * 32 B
-// and the three phases are separate warps over an NS-deep stage ring (conv_halo_ws_kernel's structure): warp 4 producer,
-// warp 5 MMA issue, warps 0-3 epilogue.
+// Warp 4 is the producer over an NS-deep stage ring; warps 0-3 (one warpgroup) issue the MMAs of a tile, release its
+// stage and run the epilogue while the producer already loads the following tiles.
 template <int C, int NA, int NB, int MODE, int NS>
-__global__ void __launch_bounds__(192) conv_s2_ws_kernel(const S2Args a, const __grid_constant__ CUtensorMap tmap_a,
+__global__ void __launch_bounds__(160) conv_s2_ws_kernel(const S2Args a, const __grid_constant__ CUtensorMap tmap_a,
                                                          const __grid_constant__ CUtensorMap tmap_b) {
   constexpr int N = NA + NB, HH = S2_TH + 1;
-  constexpr int NACC = MODE == 0 ? N : 4 * C;            // accumulator columns of one tile
+  constexpr int NQ = MODE == 0 ? 1 : 4, NW = MODE == 0 ? N : C;   // accumulators of one tile x their width
+  constexpr int NACC = NQ * NW;
   constexpr uint32_t ATOM = 8 * 128, COPY = HH * ATOM, STAGE = 4 * COPY;
   constexpr uint32_t W_BYTES = 9 * C * N * 2;
   static_assert(C == 32 && NA == 64 && NB == 64, "conv_s2_ws: 128-byte rows = (dx, c) of 32 channels / 64-channel gradients");
   extern __shared__ __align__(16) uint8_t smem_raw[];
-  __shared__ __align__(8) uint64_t full_bar[NS], empty_bar[NS], tfull_bar[2], tempty_bar[2];
-  __shared__ uint32_t tmem_slot;
+  __shared__ __align__(8) uint64_t full_bar[NS], empty_bar[NS];
+  __shared__ float stage_buf[kStageFloats];
   const uint32_t sbase = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t s_w = sbase, s_halo = s_w + W_BYTES;   // W_BYTES = 72 KB: the stages stay 1024-byte aligned
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   if (tid == 0) {
 #pragma unroll
     for (int i = 0; i < NS; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 1); }
-    mbar_init(&tfull_bar[0], 1); mbar_init(&tfull_bar[1], 1);
-    mbar_init(&tempty_bar[0], 4); mbar_init(&tempty_bar[1], 4);
     mbar_fence_init();
   }
-  if (warp == 0) tmem_alloc(&tmem_slot, 2 * NACC);
   {
     const uint4* src = reinterpret_cast<const uint4*>(a.wimg);
-    for (int v = tid; v < (int)(W_BYTES / 16); v += 192) cp_async16(s_w + (uint32_t)v * 16, src + v, true);
+    for (int v = tid; v < (int)(W_BYTES / 16); v += blockDim.x) cp_async16(s_w + (uint32_t)v * 16, src + v, true);
   }
   cp_async_commit();
   cp_async_wait<0>();
   fence_proxy_async_smem();
-  fence_before_sync();
   __syncthreads();
-  fence_after_sync();
-  const uint32_t tmem_base = tmem_slot;
   const int tiles_x = a.Wo / S2_TW, tiles_per_img = tiles_x * (a.Ho / S2_TH);
   const int first = blockIdx.x, stride = gridDim.x;
   const int my_n = first < a.ntiles ? (a.ntiles - first + stride - 1) / stride : 0;
@@ -462,85 +406,67 @@ __global__ void __launch_bounds__(192) conv_s2_ws_kernel(const S2Args a, const _
       }
     }
     __syncwarp();
-  } else if (warp == 5) {
-    if (lane == 0) {
-      for (int it = 0; it < my_n; ++it) {
-        const int st = it % NS, acc = it & 1;
-        if (it >= 2) mbar_wait(&tempty_bar[acc], ((it >> 1) - 1) & 1);
-        mbar_wait(&full_bar[st], (it / NS) & 1);
-        fence_after_sync();
-        const uint32_t sh = s_halo + (uint32_t)st * STAGE;
-        const uint32_t tacc = tmem_base + (uint32_t)(acc * NACC);
-        if (MODE == 0) {
-          constexpr uint32_t idesc = make_idesc_f16(128, N, 0, 0, kFmtF16, kFmtF16);
-          uint32_t accum = 0;
-#pragma unroll
-          for (int r = 0; r < 3; ++r)
-#pragma unroll
-            for (int s = 0; s < 3; ++s)
-#pragma unroll
-              for (int kk = 0; kk < C / 16; ++kk) {
-                const uint64_t da = make_smem_desc(sh + (s2_d(r) * 2 + s2_k(s)) * COPY + s2_k(r) * ATOM + s2_d(s) * 64 + kk * 32,
-                                                   16, ATOM, kSwizzle128B);
-                const uint64_t db = make_smem_desc(s_w + (r * 3 + s) * (C * N * 2) + 2 * kk * (N * 16), N * 16, 128,
-                                                   kNoSwizzle);
-                mma_bf16_ss(tacc, da, db, idesc, accum);
-                accum = 1;
-              }
-        } else {
-          constexpr uint32_t idesc = make_idesc_bf16(128, C, 0, 0);
-#pragma unroll
-          for (int dy = 0; dy < 2; ++dy)
-#pragma unroll
-            for (int dx = 0; dx < 2; ++dx) {
-              uint32_t accum = 0;
-#pragma unroll
-              for (int r = 0; r < 3; ++r) {
-                if (((dy + 1 - r) & 1) != 0) continue;
-#pragma unroll
-                for (int s = 0; s < 3; ++s) {
-                  if (((dx + 1 - s) & 1) != 0) continue;
-                  const int ky = (dy + 1 - r) / 2, kx = (dx + 1 - s) / 2;
-                  const int tap = (2 - r) * 3 + (2 - s);
-#pragma unroll
-                  for (int kk = 0; kk < N / 16; ++kk) {
-                    const uint64_t da = make_smem_desc(sh + ((kk / 4) * 2 + kx) * COPY + ky * ATOM + (kk % 4) * 32, 16, ATOM,
-                                                       kSwizzle128B);
-                    const uint64_t db = make_smem_desc(s_w + tap * (C * N * 2) + 2 * kk * (C * 16), C * 16, 128, kNoSwizzle);
-                    mma_bf16_ss(tacc + (uint32_t)((dy * 2 + dx) * C), da, db, idesc, accum);
-                    accum = 1;
-                  }
-                }
-              }
-            }
-        }
-        mma_commit(&empty_bar[st]);
-        mma_commit(&tfull_bar[acc]);
-      }
-    }
-    __syncwarp();
   } else {
     const int py = tid >> 3, px = tid & 7;
+    float acc_q[NQ][NW];
     for (int it = 0; it < my_n; ++it) {
-      const int acc = it & 1;
+      const int st = it % NS;
       const int tile = first + it * stride;
       const int b = tile / tiles_per_img, r = tile - b * tiles_per_img;
       const int oh0 = (r / tiles_x) * S2_TH, ow0 = (r % tiles_x) * S2_TW;
-      mbar_wait(&tfull_bar[acc], (it >> 1) & 1);
-      fence_after_sync();
-      const uint32_t taddr = tmem_base + ((uint32_t)(warp * 32) << 16) + (uint32_t)(acc * NACC);
-      uint32_t rr[NACC];
+      mbar_wait(&full_bar[st], (it / NS) & 1);
+      const uint32_t sh = s_halo + (uint32_t)st * STAGE;
+      wgmma_fence();
+      if (MODE == 0) {
+        uint32_t accum = 0;
 #pragma unroll
-      for (int col0 = 0; col0 < NACC; col0 += 32) tmem_ld32(taddr + col0, *reinterpret_cast<uint32_t(*)[32]>(&rr[col0]));
-      tmem_ld_wait();
-      fence_before_sync();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tempty_bar[acc]);
+        for (int r = 0; r < 3; ++r)
+#pragma unroll
+          for (int s = 0; s < 3; ++s)
+#pragma unroll
+            for (int kk = 0; kk < C / 16; ++kk) {
+              const uint64_t da = make_smem_desc(sh + (s2_d(r) * 2 + s2_k(s)) * COPY + s2_k(r) * ATOM + s2_d(s) * 64 + kk * 32,
+                                                 16, ATOM, kSwizzle128B);
+              const uint64_t db = make_smem_desc(s_w + (r * 3 + s) * (C * N * 2) + 2 * kk * (N * 16), N * 16, 128,
+                                                 kNoSwizzle);
+              mma128<NW, kF16>(acc_q[0], da, 8 * ATOM, db, accum);
+              accum = 1;
+            }
+      } else {
+#pragma unroll
+        for (int dy = 0; dy < 2; ++dy)
+#pragma unroll
+          for (int dx = 0; dx < 2; ++dx) {
+            uint32_t accum = 0;
+#pragma unroll
+            for (int r = 0; r < 3; ++r) {
+              if (((dy + 1 - r) & 1) != 0) continue;
+#pragma unroll
+              for (int s = 0; s < 3; ++s) {
+                if (((dx + 1 - s) & 1) != 0) continue;
+                const int ky = (dy + 1 - r) / 2, kx = (dx + 1 - s) / 2;
+                const int tap = (2 - r) * 3 + (2 - s);
+#pragma unroll
+                for (int kk = 0; kk < N / 16; ++kk) {
+                  const uint64_t da = make_smem_desc(sh + ((kk / 4) * 2 + kx) * COPY + ky * ATOM + (kk % 4) * 32, 16, ATOM,
+                                                     kSwizzle128B);
+                  const uint64_t db = make_smem_desc(s_w + tap * (C * N * 2) + 2 * kk * (C * 16), C * 16, 128, kNoSwizzle);
+                  mma128<NW, kBF16>(acc_q[(dy * 2 + dx) % NQ], da, 8 * ATOM, db, accum);
+                  accum = 1;
+                }
+              }
+            }
+          }
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+#pragma unroll
+      for (int q = 0; q < NQ; ++q) acc_fence(acc_q[q]);
+      if (tid == 0) mbar_arrive(&empty_bar[st]);   // the producer may refill this stage now
 #pragma unroll
       for (int col0 = 0; col0 < NACC; col0 += 32) {
         float v[32];
-#pragma unroll
-        for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(rr[col0 + j]);
+        acc_row32(acc_q[col0 / NW], col0 % NW, stage_buf, v);
         if (MODE == 0) {
           const size_t pix = ((size_t)b * a.Ho + oh0 + py) * a.Wo + ow0 + px;
           const bool second = col0 >= NA;
@@ -589,9 +515,6 @@ __global__ void __launch_bounds__(192) conv_s2_ws_kernel(const S2Args a, const _
       }
     }
   }
-  fence_before_sync();
-  __syncthreads();
-  if (warp == 0) tmem_dealloc(tmem_base, 2 * NACC);
 }
 
 int g_s2_ws = getenv("HB200_NO_CONV_S2_WS") ? 0 : 1;
@@ -611,8 +534,8 @@ S2EncodeFn s2_encode_fn() {
   return fn;
 }
 
-int s2_grid(const void* kern, size_t smem, int tmem_cols, int ntiles) {
-  // resident CTAs per SM from the static limits (the occupancy API under-reports these tcgen05 kernels: see conv_halo.cu)
+int s2_grid(const void* kern, size_t smem, int ntiles) {
+  // resident CTAs per SM from the static limits (registers, shared memory)
   int per_sm = 1;
   cudaFuncAttributes fa;
   if (cudaFuncGetAttributes(&fa, kern) == cudaSuccess) {
@@ -620,7 +543,6 @@ int s2_grid(const void* kern, size_t smem, int tmem_cols, int ntiles) {
     per_sm = 65536 / (((regs + 7) / 8 * 8) * 128);
     const int by_smem = (int)((size_t)(228 * 1024) / (smem + fa.sharedSizeBytes + 1024));
     if (by_smem < per_sm) per_sm = by_smem;
-    if (per_sm > 512 / tmem_cols) per_sm = 512 / tmem_cols;
     if (per_sm < 1) per_sm = 1;
   }
   const int grid = kNumSMs * per_sm;
@@ -674,7 +596,7 @@ extern "C" int hb200_conv_s2_fwd(const hb200_f16* x, const hb200_f16* wimg, hb20
   a.ntiles = batch * (a.Ho / S2_TH) * (a.Wo / S2_TW);
   constexpr int C = 32, NA = 64, NB = 64, N = NA + NB;
   constexpr size_t slab = (size_t)(((S2_TH + 1) * (S2_TW + 1) * 16 + 127) / 128 * 128);
-  const size_t smem = 9 * C * N * 2 + (4 * C / 8) * slab + 128;   // 112 KB + alignment slack: two CTAs per SM
+  const size_t smem = 9 * C * N * 2 + (4 * C / 8) * slab + 128;   // 112 KB + alignment slack
   if (g_s2_ws) {
     constexpr int NS = 2;
     const size_t smem_ws = 9 * C * N * 2 + NS * (size_t)(4 * (S2_TH + 1) * 8 * 128) + 1024;
@@ -684,8 +606,8 @@ extern "C" int hb200_conv_s2_fwd(const hb200_f16* x, const hb200_f16* wimg, hb20
       HB_CUDA(cudaFuncSetAttribute(kws, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_ws));
       attr = true;
     }
-    const int gws = kNumSMs < a.ntiles ? kNumSMs : a.ntiles;   // 208 KB of shared memory: one CTA per SM
-    kws<<<gws, 192, smem_ws, (cudaStream_t)stream>>>(a, tmap, tmap);
+    const int gws = kNumSMs < a.ntiles ? kNumSMs : a.ntiles;   // 209 KB of shared memory: one CTA per SM
+    kws<<<gws, 160, smem_ws, (cudaStream_t)stream>>>(a, tmap, tmap);
     HB_LAUNCH_OK();
     count_launch(1);
     return HB200_OK;
@@ -694,7 +616,7 @@ extern "C" int hb200_conv_s2_fwd(const hb200_f16* x, const hb200_f16* wimg, hb20
   static int grid_cache = 0;
   if (grid_cache == 0) {
     HB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    grid_cache = s2_grid((const void*)kern, smem, 2 * N, 1 << 30);
+    grid_cache = s2_grid((const void*)kern, smem, 1 << 30);
   }
   const int grid = grid_cache < a.ntiles ? grid_cache : a.ntiles;
   kern<<<grid, 128, smem, (cudaStream_t)stream>>>(a, tmap);
@@ -750,7 +672,7 @@ extern "C" int hb200_conv_s2_dgrad(const hb200_bf16* dya, const hb200_bf16* dyb,
       attr = true;
     }
     const int gws = kNumSMs < a.ntiles ? kNumSMs : a.ntiles;
-    kws<<<gws, 192, smem_ws, (cudaStream_t)stream>>>(a, ta, tb);
+    kws<<<gws, 160, smem_ws, (cudaStream_t)stream>>>(a, ta, tb);
     HB_LAUNCH_OK();
     count_launch(1);
     return HB200_OK;
@@ -759,7 +681,7 @@ extern "C" int hb200_conv_s2_dgrad(const hb200_bf16* dya, const hb200_bf16* dyb,
   static int grid_cache = 0;
   if (grid_cache == 0) {
     HB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    grid_cache = s2_grid((const void*)kern, smem, 2 * 4 * C, 1 << 30);
+    grid_cache = s2_grid((const void*)kern, smem, 1 << 30);
   }
   const int grid = grid_cache < a.ntiles ? grid_cache : a.ntiles;
   kern<<<grid, 128, smem, (cudaStream_t)stream>>>(a, ta, tb);

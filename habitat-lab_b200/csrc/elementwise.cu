@@ -3,15 +3,15 @@
 // input prep (u8/f32 gather + 2x2 mean + running mean/var), GroupNorm apply / residual / maxpool,
 // GroupNorm backward (reduce + apply), maxpool backward, dtype converts, goal/action embeddings.
 #include "common.cuh"
-#include "umma.cuh"
+#include "wgmma.cuh"
 #include <cooperative_groups.h>
 
 namespace hb200 {
 namespace cg = cooperative_groups;
-using umma::cp_async16;
-using umma::cp_async_commit;
-using umma::cp_async_wait;
-using umma::smem_u32;
+using wg::cp_async16;
+using wg::cp_async_commit;
+using wg::cp_async_wait;
+using wg::smem_u32;
 void count_launch(int n);
 
 static inline int grid_for(long long n, int bs) {
@@ -601,8 +601,8 @@ gn_bwd_apply_kernel(const grad_t* __restrict__ g, const act_t* __restrict__ act,
 // to <= 48 KB so 4+ CTAs are resident per SM and the copy / reduce / write phases of different frames overlap.
 
 // Shared tail of the cluster GroupNorm-backward kernels: per-thread partial sums (a = sum gz, bx = sum gz*x over
-// the thread's elements of channel vector `vec`) -> warp shuffle -> CTA -> cluster (DSMEM) -> dgamma/dbeta atomics
-// (cluster rank 0) -> per-group S1/S2 -> the per-channel dy coefficients c2, c3.  Ends with a cluster
+// the thread's elements of channel vector `vec`) -> warp shuffle -> CTA -> cluster (DSMEM) -> the frame's row of the
+// dgamma / dbeta partials [B][C] (cluster rank 0) -> per-group S1/S2 -> the per-channel dy coefficients c2, c3.  Ends with a cluster
 // barrier ARRIVE; the caller must execute the matching WAIT before it exits.
 __device__ __forceinline__ void gn_bwd_cluster_sums(cg::cluster_group& cluster, const GnP& p, int b, int CS, int rank,
                                                     int c0, float (&a)[8], float (&bx)[8], float* part, float* tot,
@@ -647,9 +647,9 @@ __device__ __forceinline__ void gn_bwd_cluster_sums(cg::cluster_group& cluster, 
     const float tb = r * (tx - m * ta);  // sum gz * xhat
     tot[c] = ta;
     tot[C + c] = tb;
-    if (rank == 0) {
-      atomicAdd(&dbeta[c], ta);
-      atomicAdd(&dgamma[c], tb);
+    if (rank == 0) {   // this frame's row of the dgamma / dbeta partials (summed in order by reduce_partials)
+      dbeta[(size_t)b * C + c] = ta;
+      dgamma[(size_t)b * C + c] = tb;
     }
   }
   asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");  // peers may exit once all have read
@@ -899,7 +899,7 @@ gn_pool_bwd_cluster_kernel(const grad_t* __restrict__ dpool, const uint8_t* __re
   asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
 
-// One block per frame: phase 1 reduces (dgamma/dbeta atomics + per-group sums kept in shared memory),
+// One block per frame: phase 1 reduces (the frame's dgamma / dbeta partial row + per-group sums kept in shared memory),
 // phase 2 re-reads the frame's g / y / act -- which phase 1 just pulled into L2 -- and writes dy (and
 // gz).  Compared with gn_bwd_reduce + gn_bwd_apply this removes one full HBM read of every operand, the
 // per-(frame,group) atomics and a launch + memset per layer.
@@ -962,8 +962,8 @@ gn_bwd_fused_kernel(const grad_t* __restrict__ g, const act_t* __restrict__ act,
     const int v = c >> 3, e = c & 7;
     float ta = 0.f, tb = 0.f;
     for (int q = 0; q < npl; ++q) { ta += sa[q * cv + v][e]; tb += sb[q * cv + v][e]; }
-    atomicAdd(&dbeta[c], ta);
-    atomicAdd(&dgamma[c], tb);
+    dbeta[(size_t)b * p.C + c] = ta;    // this frame's row of the partials
+    dgamma[(size_t)b * p.C + c] = tb;
     const float gm = p.gamma[c];
     ch_a[c] = gm * ta;
     ch_b[c] = gm * tb;
@@ -1070,40 +1070,35 @@ __global__ void embed_fwd_kernel(const float* __restrict__ goal, const int64_t* 
     out[(size_t)f * ld + col0 + j] = v;
   }
 }
+// One partial per (accumulator, chunk of kEmbedFrames frames), frames summed in order: deterministic.
+constexpr int kEmbedFrames = 64;
 __global__ void embed_bwd_kernel(const float* __restrict__ goal, const int64_t* __restrict__ prev_actions,
                                  const uint8_t* __restrict__ masks, const int32_t* __restrict__ rows,
                                  const float* __restrict__ d_out, int ld, int col0, int B, int n_emb,
-                                 float* __restrict__ d_w, float* __restrict__ d_b, float* __restrict__ d_emb) {
-  // block-local accumulation in smem, one atomic flush per block
-  extern __shared__ float acc[];  // [32*3 + 32 + n_emb*32]
+                                 float* __restrict__ parts) {
+  // accumulators: [0, 96) target-encoding weight (j, k), [96, 128) its bias, [128, 128 + 32 n_emb) action embedding
   const int nacc = 128 + n_emb * 32;
-  for (int i = threadIdx.x; i < nacc; i += blockDim.x) acc[i] = 0.f;
-  __syncthreads();
-  const long long total = (long long)B * 64;
-  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total;
-       i += (long long)gridDim.x * blockDim.x) {
-    const int f = (int)(i >> 6), j = (int)(i & 63);
-    const size_t row = (size_t)rows[f];
-    const float d = d_out[(size_t)f * ld + col0 + j];
-    if (j < 32) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= nacc) return;
+  const int f0 = blockIdx.y * kEmbedFrames, f1 = min(B, f0 + kEmbedFrames);
+  float v = 0.f;
+  if (i < 128) {
+    const int j = i < 96 ? i / 3 : i - 96, k = i < 96 ? i % 3 : 3;
+    for (int f = f0; f < f1; ++f) {
+      const float d = d_out[(size_t)f * ld + col0 + j];
+      if (k == 3) { v += d; continue; }
+      const size_t row = (size_t)rows[f];
       const float r = goal[row * 2], th = goal[row * 2 + 1];
-      atomicAdd(&acc[j * 3], d * r);
-      atomicAdd(&acc[j * 3 + 1], d * cosf(-th));
-      atomicAdd(&acc[j * 3 + 2], d * sinf(-th));
-      atomicAdd(&acc[96 + j], d);
-    } else {
-      const int idx = masks[f] ? (int)prev_actions[f] + 1 : 0;
-      atomicAdd(&acc[128 + idx * 32 + (j - 32)], d);
+      v += d * (k == 0 ? r : (k == 1 ? cosf(-th) : sinf(-th)));
+    }
+  } else {
+    const int idx = (i - 128) >> 5, j = (i - 128) & 31;
+    for (int f = f0; f < f1; ++f) {
+      const int fi = masks[f] ? (int)prev_actions[f] + 1 : 0;
+      if (fi == idx) v += d_out[(size_t)f * ld + col0 + 32 + j];
     }
   }
-  __syncthreads();
-  for (int i = threadIdx.x; i < nacc; i += blockDim.x) {
-    const float v = acc[i];
-    if (v == 0.f) continue;
-    if (i < 96) atomicAdd(&d_w[i], v);
-    else if (i < 128) atomicAdd(&d_b[i - 96], v);
-    else atomicAdd(&d_emb[i - 128], v);
-  }
+  parts[(size_t)blockIdx.y * nacc + i] = v;
 }
 
 
@@ -1292,7 +1287,7 @@ __global__ void rnn_shift_mask_kernel(const float* __restrict__ h_seq, const flo
 __global__ void __launch_bounds__(1024) colsum_kernel(const float* __restrict__ x, long long ld, float* __restrict__ out,
                                                       long long M, int N, int accumulate) {
   // block handles 32 columns; 32 x 32 threads stride the rows, 4 independent loads in flight per thread (the 8-row-group
-  // version walked 512 dependent loads per thread: 65 us for a 4096 x 2048 matrix); fixed summation order
+  // version walked 512 dependent loads per thread); fixed summation order
   __shared__ float red[32][33];
   const int col = blockIdx.x * 32 + (threadIdx.x & 31), ry = threadIdx.x >> 5;
   float a0 = 0.f, a1 = 0.f, a2 = 0.f, a3 = 0.f;
@@ -1549,6 +1544,54 @@ static int make_gn(GnP& p, const double* stats, const float* gamma, const float*
   p.eps = eps;
   return HB200_OK;
 }
+// ---- deterministic reduction of block partials (common.cuh) ----------------------------------------------------
+__global__ void reduce_partials_chunk_kernel(const float* __restrict__ parts, int nparts, long long ld, long long count,
+                                             int per, float* __restrict__ tmp) {
+  const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  if (i >= count) return;
+  const int p0 = blockIdx.y * per, p1 = min(nparts, p0 + per);
+  float s = 0.f;
+  for (int p = p0; p < p1; ++p) s += parts[(size_t)p * ld + i];
+  tmp[(size_t)blockIdx.y * count + i] = s;
+}
+__global__ void reduce_partials_final_kernel(const float* __restrict__ tmp, int nchunks, long long count,
+                                             float* __restrict__ dst) {
+  const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  if (i >= count) return;
+  float s = 0.f;
+  for (int k = 0; k < nchunks; ++k) s += tmp[(size_t)k * count + i];
+  dst[i] += s;
+}
+int reduce_partials(const float* parts, int nparts, long long ld, long long count, float* dst, float* tmp,
+                    cudaStream_t st) {
+  if (nparts <= 0 || count <= 0) return HB200_OK;
+  const int per = cdiv(nparts, kReduceChunks), nchunks = cdiv(nparts, per);
+  const unsigned gx = (unsigned)cdiv(count, 256);
+  reduce_partials_chunk_kernel<<<dim3(gx, nchunks), 256, 0, st>>>(parts, nparts, ld, count, per, tmp);
+  reduce_partials_final_kernel<<<gx, 256, 0, st>>>(tmp, nchunks, count, dst);
+  HB_LAUNCH_OK();
+  count_launch(2);
+  return HB200_OK;
+}
+
+// GroupNorm backward: per-frame rows of the dgamma / dbeta partials [B][C] + the reduction's scratch
+static int gn_affine_grads_workspace(cudaStream_t st, int B, int C, float** part_g, float** part_b) {
+  float* ws = nullptr;
+  int* tickets = nullptr;
+  const int rc = stream_workspace(st, (size_t)2 * B * C + (size_t)kReduceChunks * C, 0, &ws, &tickets);
+  if (rc) return rc;
+  *part_b = ws;
+  *part_g = ws + (size_t)B * C;
+  return HB200_OK;
+}
+static int gn_affine_grads_reduce(const float* part_g, const float* part_b, int B, int C, float* dgamma, float* dbeta,
+                                  cudaStream_t st) {
+  float* tmp = const_cast<float*>(part_b) + (size_t)2 * B * C;
+  const int rc = reduce_partials(part_b, B, C, C, dbeta, tmp, st);
+  if (rc) return rc;
+  return reduce_partials(part_g, B, C, C, dgamma, tmp, st);
+}
+
 }  // namespace hb200
 
 using namespace hb200;
@@ -1798,14 +1841,21 @@ extern "C" int hb200_embed_bwd(const float* goal, const int64_t* prev_actions, c
   HB_CHECK_ARG(goal && prev_actions && masks && frame_rows && d_out && d_w_tgt && d_b_tgt && d_emb && batch > 0,
                "embed_bwd: bad args");
   HB_CHECK_ARG(n_emb > 0 && n_emb <= 64, "embed_bwd: n_emb out of range");
-  const size_t smem = sizeof(float) * (128 + n_emb * 32);
-  int grid = grid_for((long long)batch * 64, 256);
-  if (grid > kNumSMs) grid = kNumSMs;
-  embed_bwd_kernel<<<grid, 256, smem, (cudaStream_t)stream>>>(goal, prev_actions, masks, frame_rows, d_out,
-                                                              ld, col0, batch, n_emb, d_w_tgt, d_b_tgt, d_emb);
+  cudaStream_t st = (cudaStream_t)stream;
+  const int nacc = 128 + n_emb * 32, nparts = cdiv(batch, kEmbedFrames);
+  float* parts = nullptr;
+  int* tickets = nullptr;
+  int rc = stream_workspace(st, (size_t)(nparts + kReduceChunks) * nacc, 0, &parts, &tickets);
+  if (rc) return rc;
+  float* tmp = parts + (size_t)nparts * nacc;
+  embed_bwd_kernel<<<dim3(cdiv(nacc, 128), nparts), 128, 0, st>>>(goal, prev_actions, masks, frame_rows, d_out, ld,
+                                                                   col0, batch, n_emb, parts);
   HB_LAUNCH_OK();
   count_launch(1);
-  return HB200_OK;
+  rc = reduce_partials(parts, nparts, nacc, 96, d_w_tgt, tmp, st);
+  if (!rc) rc = reduce_partials(parts + 96, nparts, nacc, 32, d_b_tgt, tmp, st);
+  if (!rc) rc = reduce_partials(parts + 128, nparts, nacc, (long long)n_emb * 32, d_emb, tmp, st);
+  return rc;
 }
 
 extern "C" int hb200_sensor_linear_fwd(const float* x, int in_dim, const int32_t* frame_rows, int batch, int transform,
@@ -1964,6 +2014,9 @@ extern "C" int hb200_gn_bwd(const hb200_bf16* g, const hb200_bf16* act, const hb
   HB_CHECK_ARG(mask_mode >= 0 && mask_mode <= 2 && (mask_mode != 2 || act), "gn_bwd: bad mask_mode");
   const int cv = channels / 8;
   HB_CHECK_ARG(cv >= 1 && cv <= 256 && 256 % cv == 0, "gn_bwd: C/8 = %d must divide 256", cv);
+  float *part_g = nullptr, *part_b = nullptr;
+  rc = gn_affine_grads_workspace((cudaStream_t)stream, batch, channels, &part_g, &part_b);
+  if (rc) return rc;
   if (cv <= 32) {
     // cluster path: smallest cluster whose per-CTA slice is <= 48 KB (<= 200 KB at the portable maximum of 8)
     const int ntens = mask_mode == 2 ? 3 : 2;
@@ -1993,21 +2046,21 @@ extern "C" int hb200_gn_bwd(const hb200_bf16* g, const hb200_bf16* act, const hb
   {                                                                                                          \
     auto kern = gn_bwd_cluster_kernel<m>;                                                                    \
     HB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));             \
-    HB_CUDA(cudaLaunchKernelEx(&cfg, kern, G_, A_, Y_, p, dgamma, dbeta, D_, Z_, hw, ppc));                  \
+    HB_CUDA(cudaLaunchKernelEx(&cfg, kern, G_, A_, Y_, p, part_g, part_b, D_, Z_, hw, ppc));                 \
   }
       if (mask_mode == 0) HB_GNB_CASE(0) else if (mask_mode == 1) HB_GNB_CASE(1) else HB_GNB_CASE(2)
 #undef HB_GNB_CASE
       count_launch(1);
-      return HB200_OK;
+      return gn_affine_grads_reduce(part_g, part_b, batch, channels, dgamma, dbeta, (cudaStream_t)stream);
     }
   }
   const size_t smem = sizeof(float) * (2 * (size_t)channels + 2 * (size_t)groups);
   gn_bwd_fused_kernel<<<batch, 256, smem, (cudaStream_t)stream>>>(
-      (const grad_t*)g, (const act_t*)act, (const act_t*)y, p, dgamma, dbeta,
+      (const grad_t*)g, (const act_t*)act, (const act_t*)y, p, part_g, part_b,
       (grad_t*)dy, (grad_t*)gz_out, batch, hw, mask_mode);
   HB_LAUNCH_OK();
   count_launch(1);
-  return HB200_OK;
+  return gn_affine_grads_reduce(part_g, part_b, batch, channels, dgamma, dbeta, (cudaStream_t)stream);
 }
 
 // rows per CTA for the fused stem backward: smallest cluster (1..8 CTAs per frame) whose slice fits; 0 = unsupported
@@ -2059,12 +2112,15 @@ extern "C" int hb200_gn_relu_maxpool_bwd(const hb200_bf16* dpool, const uint8_t*
   at[0].val.clusterDim.x = cs; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
   cfg.attrs = at;
   cfg.numAttrs = 1;
+  float *part_g = nullptr, *part_b = nullptr;
+  rc = gn_affine_grads_workspace((cudaStream_t)stream, batch, channels, &part_g, &part_b);
+  if (rc) return rc;
   auto kern = gn_pool_bwd_cluster_kernel;
   HB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  HB_CUDA(cudaLaunchKernelEx(&cfg, kern, (const grad_t*)dpool, argmax, (const act_t*)y, p, dgamma, dbeta,
+  HB_CUDA(cudaLaunchKernelEx(&cfg, kern, (const grad_t*)dpool, argmax, (const act_t*)y, p, part_g, part_b,
                              (grad_t*)dy, h, w, rows));
   count_launch(1);
-  return HB200_OK;
+  return gn_affine_grads_reduce(part_g, part_b, batch, channels, dgamma, dbeta, (cudaStream_t)stream);
 }
 
 extern "C" int hb200_transpose_f32(const float* src, long long ld_src, float* dst, long long ld_dst, int rows,

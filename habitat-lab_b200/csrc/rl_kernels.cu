@@ -422,10 +422,12 @@ ppo_loss_main_kernel(const float* __restrict__ feat, const float* __restrict__ w
 }
 
 // dW[a, col] = sum_b dl[b,a] * feat[b,col];  db[a] = sum_b dl[b,a]
+// One partial row per frame slab (blockIdx.y): parts[y][a * H + col] and parts[y][A1 * H + a], summed in order by
+// reduce_partials (no floating-point atomics: the result is the same every run).
 __global__ void __launch_bounds__(256)
 ppo_heads_wgrad_kernel(const float* __restrict__ feat, const float* __restrict__ dl, int B, int H,
-                       int A1, float* __restrict__ d_w_act, float* __restrict__ d_b_act,
-                       float* __restrict__ d_w_val, float* __restrict__ d_b_val) {
+                       int A1, float* __restrict__ parts) {
+  float* prow = parts + (size_t)blockIdx.y * A1 * (H + 1);
   __shared__ float red[8][kMaxA + 1][33];
   const int col = blockIdx.x * 32 + (threadIdx.x & 31);
   const int slice = threadIdx.x >> 5;  // 8 slices of the frame range of this block
@@ -442,8 +444,10 @@ ppo_heads_wgrad_kernel(const float* __restrict__ feat, const float* __restrict__
       if (a < A1) acc[a] = fmaf(dl[(size_t)b * A1 + a], x, acc[a]);
     if (blockIdx.x == 0 && (threadIdx.x & 31) < A1) bacc += dl[(size_t)b * A1 + (threadIdx.x & 31)];
   }
+  __shared__ float bred[8][32];   // bias partials of the 8 frame slices (block column 0)
 #pragma unroll
   for (int a = 0; a <= kMaxA; ++a) red[slice][a][threadIdx.x & 31] = acc[a];
+  bred[slice][threadIdx.x & 31] = bacc;
   __syncthreads();
   if (slice == 0 && col < H) {
 #pragma unroll
@@ -451,14 +455,15 @@ ppo_heads_wgrad_kernel(const float* __restrict__ feat, const float* __restrict__
       if (a < A1) {
         float s = 0.f;
         for (int w = 0; w < 8; ++w) s += red[w][a][threadIdx.x & 31];
-        float* dst = (a < A1 - 1) ? &d_w_act[(size_t)a * H + col] : &d_w_val[col];
-        atomicAdd(dst, s);
+        prow[(size_t)a * H + col] = s;
       }
     }
   }
-  if (blockIdx.x == 0 && (threadIdx.x & 31) < A1) {
+  if (blockIdx.x == 0 && slice == 0 && (threadIdx.x & 31) < A1) {
     const int a = threadIdx.x & 31;
-    atomicAdd((a < A1 - 1) ? &d_b_act[a] : d_b_val, bacc);
+    float sb = 0.f;
+    for (int w = 0; w < 8; ++w) sb += bred[w][a];
+    prow[(size_t)A1 * H + a] = sb;
   }
 }
 
@@ -541,10 +546,22 @@ extern "C" int hb200_ppo_loss(const float* features, const float* w_act, const f
     HB_CUDA(cudaMemsetAsync(d_w_val, 0, sizeof(float) * hidden, st));
     HB_CUDA(cudaMemsetAsync(d_b_val, 0, sizeof(float), st));
     dim3 g(cdiv(hidden, 32), min(32, cdiv(batch, 64)));
-    ppo_heads_wgrad_kernel<<<g, 256, 0, st>>>(features, dl, batch, hidden, n_actions + 1, d_w_act,
-                                              d_b_act, d_w_val, d_b_val);
+    const int A1 = n_actions + 1;
+    const long long row = (long long)A1 * (hidden + 1);   // one partial row per frame slab
+    float* parts = nullptr;
+    int* tickets = nullptr;
+    int rc = stream_workspace(st, (size_t)(g.y + kReduceChunks) * row, 0, &parts, &tickets);
+    if (rc) return rc;
+    float* tmp = parts + (size_t)g.y * row;
+    ppo_heads_wgrad_kernel<<<g, 256, 0, st>>>(features, dl, batch, hidden, A1, parts);
     HB_LAUNCH_OK();
     count_launch(1);
+    const long long H = hidden;
+    rc = reduce_partials(parts, g.y, row, (long long)n_actions * H, d_w_act, tmp, st);
+    if (!rc) rc = reduce_partials(parts + (size_t)n_actions * H, g.y, row, H, d_w_val, tmp, st);
+    if (!rc) rc = reduce_partials(parts + (size_t)A1 * H, g.y, row, n_actions, d_b_act, tmp, st);
+    if (!rc) rc = reduce_partials(parts + (size_t)A1 * H + n_actions, g.y, row, 1, d_b_val, tmp, st);
+    if (rc) return rc;
   }
   return HB200_OK;
 }

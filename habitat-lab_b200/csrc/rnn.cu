@@ -405,7 +405,7 @@ lstm_seq_bwd_kernel(const float* __restrict__ dh_out, const float* __restrict__ 
 // =====================================================================================
 // v2 of the persistent LSTM kernels (hidden = 512): register-tiled recurrent mat-vecs.
 // v1 gives every sequence its own warp, so each W_hh element is re-read from shared memory once per sequence and
-// the step is bound by shared-memory bandwidth (1 LDS per FMA: ~4.3 us of the ~7.7 us step).  Here a warp owns an
+// the step is bound by shared-memory bandwidth (1 LDS per FMA).  Here a warp owns an
 // 8-sequence x 8-gate-row (forward) / 8-sequence x 4-column (backward) tile: one 16-byte LDS feeds 8 x 4 FMAs, the
 // staged h_{t-1} block / the streamed dgates rows are shared by the whole tile, and the 64 (32) per-lane partial
 // sums are finished with one transpose-reduce.

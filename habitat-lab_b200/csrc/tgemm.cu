@@ -1,45 +1,30 @@
-// hb200 -- TF32 tensor-core GEMM (tcgen05 kind::tf32) on fp32 operands for the dense layers:
+// hb200 -- TF32 tensor-core GEMM (wgmma .tf32) on fp32 operands for the dense layers:
 // visual_fc, the LSTM input projections and their data / weight gradients.
 //
 //   C[M,N] (f32) (+)= A[M,K] * B[K,N] (+ bias[N]) (ReLU)
 //   A(m,k) = a[m*a_ms + k*a_ks],  B(k,n) = b[k*b_ks + n*b_ns]   (one of the two strides of each == 1)
 //
 // Precision: operands are fp32 in memory; the tensor core reads them as TF32 (10-bit mantissa,
-// the reference's own cuDNN-RNN precision on CUDA), accumulation is fp32 in TMEM.
+// the reference's own cuDNN-RNN precision on CUDA), accumulation is fp32 in the warpgroup's registers.
 //
-// Operand tiles are copied with 16-byte cp.async (4 floats) straight into the no-swizzle UMMA
-// layouts (descriptor encodings pinned by hb200_umma_gemm_probe):
-//   K-major  (k contiguous):  vector (row, k4) at k4*rows*16 + row*16          LBO = rows*16, SBO = 128
-//   MN-major (mn contiguous): vector (mn4, k)  at (k>>3)*LBO + mn4*128 + (k&7)*16,  SBO = 128 (next 4 mn),
-//                             LBO = (rows/4)*128 (next 8 k)
+// wgmma reads tf32 operands K-major only: both operands are [rows][k] tiles in the 128-byte-swizzle layout, copied with
+// 16-byte cp.async (4 floats) or one TMA box per operand and chunk.
 // One MMA covers K = 8 (32 bytes); a chunk is K = 32 (4 MMAs); 3-stage cp.async ring as in conv.cu.
-// Weight gradients (K = frames, tiny M x N tile grid) are split over K with fp32 atomics.
+// Weight gradients (K = frames, tiny M x N tile grid) are split over K; the splits are summed in order (deterministic).
 #include <cuda.h>
 #include "common.cuh"
 #include <stdlib.h>
 #include <map>
 #include <mutex>
-#include "umma.cuh"
+#include "wgmma.cuh"
 
 namespace hb200 {
 void count_launch(int n);
-using namespace umma;
+using namespace wg;
 
 constexpr int GT_M = 128, GT_K = 32, GT_STAGES = 3;
 
-__host__ __device__ constexpr uint32_t make_idesc_tf32(int M, int N, int a_mn, int b_mn) {
-  return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)a_mn << 15) | ((uint32_t)b_mn << 16) |
-         ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-__device__ __forceinline__ void mma_tf32_ss(uint32_t tmem_d, uint64_t da, uint64_t db, uint32_t idesc, uint32_t acc) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t"
-      "}\n" ::"r"(tmem_d), "l"(da), "l"(db), "r"(idesc), "r"(acc)
-      : "memory");
-}
+constexpr uint32_t GT_A_HI = 8 * 1024;   // rows 0 -> 64 of a swizzled K-major tile
 
 struct TgemmArgs {
   const float* a; long long a_ms, a_ks;
@@ -54,69 +39,46 @@ struct TgemmArgs {
   int vec4;   // c, ldc (and bias) allow 16-byte accesses
 };
 
-// load one [ROWS x 32] operand tile (rows = m or n, zero-filled out of range)
-template <int MNMAJOR>
-__device__ __forceinline__ void tg_load(const float* __restrict__ p, long long s_mn, long long s_k, int mn0, int MN,
-                                        int k0, int k_end, uint32_t sdst, int rows) {
-  if (!MNMAJOR) {
-    // K-major: vector = 4 consecutive k of one row; 8 vectors per row per chunk
-    // 128-byte swizzle: 8 consecutive threads fetch the 8 x 16 B of one row (a full 128-byte line) and write one
-    // swizzled shared-memory row (conflict free); the row-per-thread mapping of the no-swizzle layout touched 32
-    // different lines per request and used half of every 32-byte sector.
-    for (int v = threadIdx.x; v < rows * 8; v += 128) {
-      const int row = v >> 3, k4 = v & 7;
-      const int gm = mn0 + row, gk = k0 + k4 * 4;
-      const bool ok = gm < MN && gk + 3 < k_end;
-      const float* g = ok ? p + (long long)gm * s_mn + gk : p;
-      cp_async16(sdst + (uint32_t)((row >> 3) << 10) + (uint32_t)((row & 7) << 7) + (uint32_t)((k4 ^ (row & 7)) << 4),
-                 g, ok);
-    }
-  } else {
-    // MN-major: vector = 4 consecutive mn at one k; rows/4 vectors per k
-    const int r4 = rows >> 2;
-    for (int v = threadIdx.x; v < r4 * GT_K; v += 128) {
-      // 8 consecutive threads = the 8 k rows of one core matrix (128 contiguous smem bytes), the next
-      // 8 threads the next 4 mn (adjacent 16 B in global memory)
-      const int kl = v & 7, mb = (v >> 3) % r4, k = (v / (8 * r4)) * 8 + kl;
-      const int gm = mn0 + mb * 4, gk = k0 + k;
-      const bool ok = gm + 3 < MN && gk < k_end;
-      const float* g = ok ? p + (long long)gk * s_k + gm : p;
-      cp_async16(sdst + (uint32_t)(k >> 3) * (r4 * 128) + (uint32_t)mb * 128 + (uint32_t)(k & 7) * 16, g, ok);
-    }
+// load one K-major [ROWS x 32] operand tile (rows = m or n, zero-filled out of range)
+// vector = 4 consecutive k of one row; 8 vectors per row per chunk.  128-byte swizzle: 8 consecutive threads fetch the
+// 8 x 16 B of one row (a full 128-byte line) and write one swizzled shared-memory row (conflict free).
+__device__ __forceinline__ void tg_load(const float* __restrict__ p, long long s_mn, int mn0, int MN, int k0, int k_end,
+                                        uint32_t sdst, int rows) {
+  for (int v = threadIdx.x; v < rows * 8; v += 128) {
+    const int row = v >> 3, k4 = v & 7;
+    const int gm = mn0 + row, gk = k0 + k4 * 4;
+    const bool ok = gm < MN && gk + 3 < k_end;
+    const float* g = ok ? p + (long long)gm * s_mn + gk : p;
+    cp_async16(sdst + (uint32_t)((row >> 3) << 10) + (uint32_t)((row & 7) << 7) + (uint32_t)((k4 ^ (row & 7)) << 4),
+               g, ok);
   }
 }
 
-// TMEM accumulator tile -> C: shared by the cp.async and the TMA kernels.  Plain launches add bias / accumulate / ReLU
-// here; split-K launches either add their partial with fp32 atomics (weight gradients) or park it in the workspace
-// for the ticketed, in-order reduction of the skinny path.
+// accumulator tile -> C: shared by the cp.async and the TMA kernels.  Plain launches add bias / accumulate / ReLU
+// here; split-K launches park their partial in the workspace for the ticketed reduction in split order (the same
+// sum every run).
 template <int BN>
-__device__ __forceinline__ void tg_epilogue(const TgemmArgs& a, uint32_t tmem_base, int m0, int n0) {
-  constexpr uint32_t kTmemCols = BN < 32 ? 32 : BN;
-  const int tid = threadIdx.x, warp = tid >> 5;
-  const uint32_t taddr = tmem_base + ((uint32_t)(warp * 32) << 16);
+__device__ __forceinline__ void tg_epilogue(const TgemmArgs& a, float (&acc_t)[BN], float* stage_buf, int m0, int n0) {
+  const int tid = threadIdx.x;
   const int m = m0 + tid;
+  acc_fence(acc_t);
   if (a.ws) {
     __shared__ int s_last;
     float* wrow = a.ws + ((size_t)blockIdx.z * a.M + m) * a.N + n0;
-#pragma unroll 1
+#pragma unroll
     for (int col0 = 0; col0 < BN; col0 += 32) {
-      uint32_t r[32];
-      tmem_ld32(taddr + col0, r);
-      tmem_ld_wait();
+      float r[32];
+      acc_row32(acc_t, col0, stage_buf, r);
       if (m < a.M) {
 #pragma unroll
         for (int j = 0; j < 32; j += 4) {
           if (n0 + col0 + j < a.N)   // N % 4 == 0
-            __stcg(reinterpret_cast<float4*>(wrow + col0 + j),
-                   make_float4(__uint_as_float(r[j]), __uint_as_float(r[j + 1]), __uint_as_float(r[j + 2]),
-                               __uint_as_float(r[j + 3])));
+            __stcg(reinterpret_cast<float4*>(wrow + col0 + j), make_float4(r[j], r[j + 1], r[j + 2], r[j + 3]));
         }
       }
     }
-    fence_before_sync();
     __threadfence();
     __syncthreads();
-    if (warp == 0) tmem_dealloc(tmem_base, kTmemCols);
     const int tile = blockIdx.y * gridDim.x + blockIdx.x;
     if (tid == 0) s_last = (atomicAdd(&a.tickets[tile], 1) == (int)gridDim.z - 1);
     __syncthreads();
@@ -145,20 +107,18 @@ __device__ __forceinline__ void tg_epilogue(const TgemmArgs& a, uint32_t tmem_ba
     if (tid == 0) a.tickets[tile] = 0;   // ready for the next launch on this stream
     return;
   }
-#pragma unroll 1
+#pragma unroll
   for (int col0 = 0; col0 < BN; col0 += 32) {
-    uint32_t r[32];
-    tmem_ld32(taddr + col0, r);
-    tmem_ld_wait();
-    if (m < a.M && gridDim.z == 1 && a.vec4) {
+    float r[32];
+    acc_row32(acc_t, col0, stage_buf, r);
+    if (m < a.M && a.vec4) {   // (split-K launches always take the workspace path above)
       // one thread owns 128 contiguous bytes of its row: float4 stores (N % 4 == 0: a group of 4 is in or out)
       float* dst = a.c + (long long)m * a.ldc + n0 + col0;
 #pragma unroll
       for (int j = 0; j < 32; j += 4) {
         const int n = n0 + col0 + j;
         if (n >= a.N) continue;
-        float4 v = make_float4(__uint_as_float(r[j]), __uint_as_float(r[j + 1]), __uint_as_float(r[j + 2]),
-                               __uint_as_float(r[j + 3]));
+        float4 v = make_float4(r[j], r[j + 1], r[j + 2], r[j + 3]);
         if (a.bias) {
           const float4 b4 = *reinterpret_cast<const float4*>(a.bias + n);
           v.x += b4.x; v.y += b4.y; v.z += b4.z; v.w += b4.w;
@@ -170,78 +130,41 @@ __device__ __forceinline__ void tg_epilogue(const TgemmArgs& a, uint32_t tmem_ba
         if (a.relu) { v.x = fmaxf(v.x, 0.f); v.y = fmaxf(v.y, 0.f); v.z = fmaxf(v.z, 0.f); v.w = fmaxf(v.w, 0.f); }
         *reinterpret_cast<float4*>(dst + j) = v;
       }
-    } else if (m < a.M && a.vec4) {
-      // split-K partial: 16-byte reductions (red.global.add.v4.f32), a quarter of the scalar atomics' L2 operations
-      float* dst = a.c + (long long)m * a.ldc + n0 + col0;
-#pragma unroll
-      for (int j = 0; j < 32; j += 4) {
-        const int n = n0 + col0 + j;
-        if (n >= a.N) continue;
-        float4 v = make_float4(__uint_as_float(r[j]), __uint_as_float(r[j + 1]), __uint_as_float(r[j + 2]),
-                               __uint_as_float(r[j + 3]));
-        if (a.bias && blockIdx.z == 0) {
-          const float4 b4 = *reinterpret_cast<const float4*>(a.bias + n);
-          v.x += b4.x; v.y += b4.y; v.z += b4.z; v.w += b4.w;
-        }
-        atomicAdd(reinterpret_cast<float4*>(dst + j), v);
-      }
     } else if (m < a.M) {
       float* dst = a.c + (long long)m * a.ldc + n0 + col0;
 #pragma unroll
       for (int j = 0; j < 32; ++j) {
         const int n = n0 + col0 + j;
         if (n >= a.N) continue;
-        float v = __uint_as_float(r[j]);
-        if (gridDim.z > 1) {
-          if (a.bias && blockIdx.z == 0) v += a.bias[n];
-          atomicAdd(dst + j, v);
-        } else {
-          if (a.bias) v += a.bias[n];
-          if (a.accumulate) v += dst[j];
-          if (a.relu) v = fmaxf(v, 0.f);
-          dst[j] = v;
-        }
+        float v = r[j];
+        if (a.bias) v += a.bias[n];
+        if (a.accumulate) v += dst[j];
+        if (a.relu) v = fmaxf(v, 0.f);
+        dst[j] = v;
       }
     }
   }
-  fence_before_sync();
-  __syncthreads();
-  if (warp == 0) tmem_dealloc(tmem_base, kTmemCols);
 }
 
 // NST = cp.async ring depth: 3 for the learner's many-CTA launches, deeper for the skinny (few CTAs, latency-bound) path
-template <int BN, int A_MN, int B_MN, int NST = GT_STAGES>
+template <int BN, int NST = GT_STAGES>
 __global__ void __launch_bounds__(128) tgemm_kernel(const TgemmArgs a) {
   extern __shared__ __align__(16) uint8_t smem_raw[];
-  __shared__ __align__(8) uint64_t mma_bar[NST];
-  __shared__ uint32_t tmem_slot;
+  __shared__ float stage_buf[kStageFloats];
   constexpr uint32_t kABytes = GT_M * GT_K * 4, kBBytes = BN * GT_K * 4, kStage = kABytes + kBBytes;
-  constexpr uint32_t kTmemCols = BN < 32 ? 32 : BN;
   const uint32_t sbase = (smem_u32(smem_raw) + 1023u) & ~1023u;  // swizzle atoms are 1024-byte aligned
-  const int tid = threadIdx.x, warp = tid >> 5;
   const int m0 = blockIdx.y * GT_M, n0 = blockIdx.x * BN;
   const int k_begin = blockIdx.z * a.k_per_split;
   const int k_end = min(a.K, k_begin + a.k_per_split);
   const int nchunks = (k_end - k_begin + GT_K - 1) / GT_K;
   if (nchunks <= 0) return;
-
-  if (tid == 0) {
-#pragma unroll
-    for (int s = 0; s < NST; ++s) mbar_init(&mma_bar[s], 1);
-    mbar_fence_init();
-  }
-  if (warp == 0) tmem_alloc(&tmem_slot, kTmemCols);
-  fence_before_sync();
-  __syncthreads();
-  fence_after_sync();
-  const uint32_t tmem_base = tmem_slot;
-  constexpr uint32_t idesc = make_idesc_tf32(GT_M, BN, A_MN, B_MN);
+  float acc_t[BN];
 
   auto load_chunk = [&](int c, int st) {
     const uint32_t sa = sbase + st * kStage, sb = sa + kABytes;
     const int k0 = k_begin + c * GT_K;
-    tg_load<A_MN>(a.a, a.a_ms, a.a_ks, m0, a.M, k0, k_end, sa, GT_M);
-    tg_load<B_MN>(a.b, a.b_ns, a.b_ks, n0, a.N, k0, k_end, sb, BN);
+    tg_load(a.a, a.a_ms, m0, a.M, k0, k_end, sa, GT_M);
+    tg_load(a.b, a.b_ns, n0, a.N, k0, k_end, sb, BN);
   };
 #pragma unroll
   for (int c = 0; c < NST - 1; ++c) {
@@ -253,51 +176,43 @@ __global__ void __launch_bounds__(128) tgemm_kernel(const TgemmArgs a) {
     cp_async_wait<NST - 2>();
     fence_proxy_async_smem();
     __syncthreads();
-    if (tid == 0) {
-      fence_after_sync();
+    {
       const uint32_t sa = sbase + st * kStage, sb = sa + kABytes;
+      wgmma_fence();
 #pragma unroll
-      for (int kk = 0; kk < GT_K / 8; ++kk) {
-        // K-major: the two 16-byte k4 vectors of this K=8 step are LBO = rows*16 apart
-        // MN-major: one 8-k block per step, blocks LBO' = (rows/4)*128 apart; SBO = 128 between 4-mn vectors
-        const uint64_t da = A_MN ? make_smem_desc(sa + kk * (GT_M / 4) * 128, (GT_M / 4) * 128, 128, kNoSwizzle)
-                                 : make_smem_desc(sa + kk * 32, 16, 1024, kSwizzle128B);
-        const uint64_t db = B_MN ? make_smem_desc(sb + kk * (BN / 4) * 128, (BN / 4) * 128, 128, kNoSwizzle)
-                                 : make_smem_desc(sb + kk * 32, 16, 1024, kSwizzle128B);
-        mma_tf32_ss(tmem_base, da, db, idesc, (c > 0 || kk > 0) ? 1u : 0u);
-      }
-      mma_commit(&mma_bar[st]);
+      for (int kk = 0; kk < GT_K / 8; ++kk)
+        mma128<BN, kTF32>(acc_t, make_smem_desc(sa + kk * 32, 16, 1024, kSwizzle128B), GT_A_HI,
+                          make_smem_desc(sb + kk * 32, 16, 1024, kSwizzle128B), (c > 0 || kk > 0) ? 1u : 0u);
+      wgmma_commit();
     }
     const int nc = c + NST - 1;
     if (nc < nchunks) {
-      if (c >= 1) mbar_wait(&mma_bar[(c - 1) % NST], ((c - 1) / NST) & 1);
+      wgmma_wait<1>();   // the MMAs of chunk c-1 have read stage nc % NST
       load_chunk(nc, nc % NST);
     }
     cp_async_commit();
   }
-  mbar_wait(&mma_bar[(nchunks - 1) % NST], ((nchunks - 1) / NST) & 1);
-  fence_after_sync();
-
-  tg_epilogue<BN>(a, tmem_base, m0, n0);
+  wgmma_wait<0>();
+  tg_epilogue<BN>(a, acc_t, stage_buf, m0, n0);
 }
 
 // ---- TMA-fed variant ---------------------------------------------------------------------------------------------------
-// The cp.async kernel above spends ~4000 cycles per K chunk on 2048 LDGSTS + their addresses (the tensor core needs 256):
-// 54 TFLOP/s on the learner's dense layers.  Here one thread issues two TMA box loads per chunk ([32 k] x [128 | BN rows],
-// SWIZZLE_128B = the K-major operand layout, out-of-range rows / k zero-filled by the TMA unit), one thread issues the
-// MMAs, and the ring is ordered by full (transaction-count) / empty (tcgen05.commit) barriers.
+// The cp.async kernel above spends far more issue slots per K chunk on 2048 LDGSTS + their addresses than the tensor core
+// needs for the chunk: the LSU work, not the tensor core, bounds it.  Here one thread issues two TMA box loads per chunk ([32 k] x [128 | BN
+// rows], SWIZZLE_128B = the K-major operand layout, out-of-range rows / k zero-filled by the TMA unit) into an NST-deep
+// ring ordered by full (transaction-count) barriers; the warpgroup refills a stage once wgmma.wait_group says the
+// MMAs that read it have completed.
 template <int BN, int NST>
 __global__ void __launch_bounds__(128) tgemm_tma_kernel(const TgemmArgs a, const __grid_constant__ CUtensorMap tmap_a,
                                                         const __grid_constant__ CUtensorMap tmap_b) {
   extern __shared__ __align__(16) uint8_t smem_raw[];
-  __shared__ __align__(8) uint64_t full_bar[NST], empty_bar[NST], done_bar;
-  __shared__ uint32_t tmem_slot;
+  __shared__ __align__(8) uint64_t full_bar[NST];
+  __shared__ float stage_buf[kStageFloats];
   constexpr uint32_t kABytes = GT_M * GT_K * 4, kBBytes = BN * GT_K * 4, kStage = kABytes + kBBytes;
-  constexpr uint32_t kTmemCols = BN < 32 ? 32 : BN;
   const CUtensorMap* const pa = &tmap_a;   // param-space addresses, taken in the kernel body
   const CUtensorMap* const pb = &tmap_b;
   const uint32_t sbase = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int tid = threadIdx.x;
   const int m0 = blockIdx.y * GT_M, n0 = blockIdx.x * BN;
   const int k_begin = blockIdx.z * a.k_per_split;
   const int k_end = min(a.K, k_begin + a.k_per_split);
@@ -305,58 +220,51 @@ __global__ void __launch_bounds__(128) tgemm_tma_kernel(const TgemmArgs a, const
   if (nchunks <= 0) return;
   if (tid == 0) {
 #pragma unroll
-    for (int s = 0; s < NST; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-    mbar_init(&done_bar, 1);
+    for (int s = 0; s < NST; ++s) mbar_init(&full_bar[s], 1);
     mbar_fence_init();
   }
-  if (warp == 0) tmem_alloc(&tmem_slot, kTmemCols);
-  fence_before_sync();
   __syncthreads();
-  fence_after_sync();
-  const uint32_t tmem_base = tmem_slot;
-  constexpr uint32_t idesc = make_idesc_tf32(GT_M, BN, 0, 0);
-  if (warp == 0) {
-    if (lane == 0) {
-      for (int c = 0; c < nchunks; ++c) {
-        const int st = c % NST;
-        if (c >= NST) mbar_wait(&empty_bar[st], ((c / NST) - 1) & 1);
-        const uint32_t sa = sbase + st * kStage;
-        mbar_expect_tx(&full_bar[st], kStage);
-        tma_load_2d(sa, pa, &full_bar[st], k_begin + c * GT_K, m0);
-        tma_load_2d(sa + kABytes, pb, &full_bar[st], k_begin + c * GT_K, n0);
-      }
+  if (tid == 0) {
+    for (int c = 0; c < NST && c < nchunks; ++c) {
+      const uint32_t sa = sbase + c * kStage;
+      mbar_expect_tx(&full_bar[c], kStage);
+      tma_load_2d(sa, pa, &full_bar[c], k_begin + c * GT_K, m0);
+      tma_load_2d(sa + kABytes, pb, &full_bar[c], k_begin + c * GT_K, n0);
     }
-    __syncwarp();
-  } else if (warp == 1) {
-    if (lane == 0) {
-      for (int c = 0; c < nchunks; ++c) {
-        const int st = c % NST;
-        mbar_wait(&full_bar[st], (c / NST) & 1);
-        fence_after_sync();
-        const uint32_t sa = sbase + st * kStage, sb = sa + kABytes;
-#pragma unroll
-        for (int kk = 0; kk < GT_K / 8; ++kk)
-          mma_tf32_ss(tmem_base, make_smem_desc(sa + kk * 32, 16, 1024, kSwizzle128B),
-                      make_smem_desc(sb + kk * 32, 16, 1024, kSwizzle128B), idesc, (c > 0 || kk > 0) ? 1u : 0u);
-        mma_commit(&empty_bar[st]);
-      }
-      mma_commit(&done_bar);
-    }
-    __syncwarp();
   }
-  mbar_wait(&done_bar, 0);
-  fence_after_sync();
-  tg_epilogue<BN>(a, tmem_base, m0, n0);
+  float acc_t[BN];
+  for (int c = 0; c < nchunks; ++c) {
+    const int st = c % NST;
+    mbar_wait(&full_bar[st], (c / NST) & 1);
+    const uint32_t sa = sbase + st * kStage, sb = sa + kABytes;
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < GT_K / 8; ++kk)
+      mma128<BN, kTF32>(acc_t, make_smem_desc(sa + kk * 32, 16, 1024, kSwizzle128B), GT_A_HI,
+                        make_smem_desc(sb + kk * 32, 16, 1024, kSwizzle128B), (c > 0 || kk > 0) ? 1u : 0u);
+    wgmma_commit();
+    wgmma_wait<1>();   // the MMAs of chunk c-1 are done: refill its stage with chunk c-1+NST
+    const int nc = c - 1 + NST;
+    if (tid == 0 && c >= 1 && nc < nchunks) {
+      const int ps = (c - 1) % NST;
+      const uint32_t pa_s = sbase + ps * kStage;
+      mbar_expect_tx(&full_bar[ps], kStage);
+      tma_load_2d(pa_s, pa, &full_bar[ps], k_begin + nc * GT_K, m0);
+      tma_load_2d(pa_s + kABytes, pb, &full_bar[ps], k_begin + nc * GT_K, n0);
+    }
+  }
+  wgmma_wait<0>();
+  tg_epilogue<BN>(a, acc_t, stage_buf, m0, n0);
 }
 }  // namespace hb200
 
 using namespace hb200;
 
-// workspace of the skinny split-K path: one per stream (launches on a stream are ordered; two streams never share one),
+// per-stream scratch (split-K partials of the skinny path, the block partials of reduce_partials): one per stream (launches on a stream are ordered; two streams never share one),
 // and one per CUDA-graph capture (keyed by the capture id: the graph keeps using its buffers after the capturing stream
 // has gone back to the pool).  Under capture the allocation runs in relaxed capture mode -- cudaMalloc is not a stream
 // operation -- and the ticket memset becomes the graph's first node (tickets are zero between launches anyway).
-static int skinny_workspace(cudaStream_t st, size_t floats, int tiles, float** ws, int** tickets) {
+int hb200::stream_workspace(cudaStream_t st, size_t floats, int tiles, float** ws, int** tickets) {
   struct Ws { float* buf = nullptr; size_t cap = 0; int* tickets = nullptr; };
   static std::mutex mu;
   static std::map<unsigned long long, Ws> table;
@@ -451,8 +359,7 @@ extern "C" int hb200_tgemm(const float* a, long long a_ms, long long a_ks, const
                            long long b_ns, float* c, long long ldc, const float* bias, int m, int n, int k,
                            int accumulate, int relu, hb200_stream_t stream) {
   HB_CHECK_ARG(a && b && c && m > 0 && n > 0 && k > 0, "tgemm: bad args");
-  // MN-major fp32 operands would need the SWIZZLE_128B_BASE32B layouts (the plain interleaved MN-major
-  // descriptor is 16-bit only: verified wrong on hardware) -> K-major only, callers transpose
+  // wgmma reads tf32 operands K-major only -> callers transpose
   HB_CHECK_ARG(a_ks == 1 && b_ks == 1, "tgemm: both operands must be K-major (a_ks == 1, b_ks == 1)");
   const int a_mn = (a_ks == 1) ? 0 : 1;   // k contiguous -> K-major
   const int b_mn = (b_ks == 1) ? 0 : 1;
@@ -461,15 +368,11 @@ extern "C" int hb200_tgemm(const float* a, long long a_ms, long long a_ks, const
   HB_CHECK_ARG(lda % 4 == 0 && ldb % 4 == 0 && ((uintptr_t)a & 15) == 0 && ((uintptr_t)b & 15) == 0,
                "tgemm: operands must be 16-byte aligned with leading dimensions that are multiples of 4");
   HB_CHECK_ARG(k % 4 == 0 && (!a_mn || m % 4 == 0) && (!b_mn || n % 4 == 0), "tgemm: k (and mn-major extents) must be multiples of 4");
-  int BN = n >= 256 ? 256 : (n >= 128 ? 128 : (n >= 64 ? 64 : 32));
+  // N tile <= 128: a 128 x 128 fp32 accumulator is 128 registers per thread of the warpgroup
+  int BN = n >= 128 ? 128 : (n >= 64 ? 64 : 32);
   {
-    // N tile 128 instead of 256 when that is what fills the 148 SMs (2 CTAs per SM fit at 96 KB of stages)
     static const int forced = getenv("HB200_TGEMM_BN") ? atoi(getenv("HB200_TGEMM_BN")) : 0;
-    if (forced == 32 || forced == 64 || forced == 128 || forced == 256) {
-      if (forced <= BN) BN = forced;
-    } else if (BN == 256 && (long long)cdiv(n, 256) * cdiv(m, GT_M) < 2 * kNumSMs) {
-      BN = 128;
-    }
+    if ((forced == 32 || forced == 64 || forced == 128) && forced <= BN) BN = forced;
   }
   HB_CHECK_ARG(n % 4 == 0, "tgemm: n must be a multiple of 4");
   TgemmArgs g;
@@ -480,7 +383,7 @@ extern "C" int hb200_tgemm(const float* a, long long a_ms, long long a_ks, const
   cudaStream_t st = (cudaStream_t)stream;
   if (m <= GT_M && k >= 256 && cdiv(n, BN) < kNumSMs / 2 && !a_mn && !b_mn) {
     // one row tile (the actor: 64 frames): a handful of CTAs would each walk the whole K, one DRAM latency per
-    // 32-wide chunk (77 us for visual_fc at K = 2048).  32-wide N tiles x K splits of >= 4 chunks put one CTA on every SM,
+    // 32-wide chunk.  32-wide N tiles x K splits of >= 4 chunks put one CTA on every SM,
     // each with a deep cp.async ring; partial tiles meet in an L2-resident workspace and the last CTA of each tile
     // reduces them in split order (8 KB per split).
     BN = 32;
@@ -493,14 +396,14 @@ extern "C" int hb200_tgemm(const float* a, long long a_ms, long long a_ks, const
     const int kps = ((cdiv(k, sp) + GT_K - 1) / GT_K) * GT_K;
     sp = cdiv(k, kps);
     if (sp > 1) {
-      int rc = skinny_workspace(st, (size_t)sp * m * n, nt, &g.ws, &g.tickets);
+      int rc = stream_workspace(st, (size_t)sp * m * n, nt, &g.ws, &g.tickets);
       if (rc) return rc;
     }
     g.k_per_split = kps;
     dim3 grid(nt, 1, sp);
     if (g_tgemm_tma) return launch_tgemm_tma<32, kDeep>(g, grid, st);
     const size_t smem = (size_t)kDeep * (GT_M * GT_K * 4 + 32 * GT_K * 4) + 1024;
-    auto kern = tgemm_kernel<32, 0, 0, kDeep>;
+    auto kern = tgemm_kernel<32, kDeep>;
     HB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     kern<<<grid, 128, smem, st>>>(g);
     HB_LAUNCH_OK();
@@ -516,6 +419,10 @@ extern "C" int hb200_tgemm(const float* a, long long a_ms, long long a_ks, const
   }
   g.k_per_split = ((cdiv(k, splits) + GT_K - 1) / GT_K) * GT_K;
   splits = cdiv(k, g.k_per_split);
+  if (splits > 1) {   // partial tiles meet in the workspace and are summed in split order (deterministic)
+    int rc = stream_workspace(st, (size_t)splits * m * n, (int)tiles, &g.ws, &g.tickets);
+    if (rc) return rc;
+  }
   dim3 grid(cdiv(n, BN), cdiv(m, GT_M), splits);
   if (g_tgemm_tma && !a_mn && !b_mn) {
     // ring depth: two CTAs per SM (3 x 32 KB stages) when there are enough tiles for that, else one CTA with a deep ring
@@ -523,29 +430,21 @@ extern "C" int hb200_tgemm(const float* a, long long a_ms, long long a_ks, const
     switch (BN) {
       case 32: return launch_tgemm_tma<32, 4>(g, grid, st);
       case 64: return launch_tgemm_tma<64, 4>(g, grid, st);
-      case 128: return ctas > kNumSMs ? launch_tgemm_tma<128, 3>(g, grid, st) : launch_tgemm_tma<128, 6>(g, grid, st);
-      default: return launch_tgemm_tma<256, 4>(g, grid, st);
+      default: return ctas > kNumSMs ? launch_tgemm_tma<128, 3>(g, grid, st) : launch_tgemm_tma<128, 6>(g, grid, st);
     }
   }
-#define HB_TG(bn, AM, BM)                                                                          \
+#define HB_TG(bn)                                                                                  \
   {                                                                                                \
     const size_t smem = (size_t)GT_STAGES * (GT_M * GT_K * 4 + bn * GT_K * 4) + 1024;              \
-    auto kern = tgemm_kernel<bn, AM, BM>;                                                          \
+    auto kern = tgemm_kernel<bn>;                                                                  \
     HB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));   \
     kern<<<grid, 128, smem, st>>>(g);                                                              \
   }
-#define HB_TG_BN(AM, BM)                 \
-  switch (BN) {                          \
-    case 32: HB_TG(32, AM, BM); break;   \
-    case 64: HB_TG(64, AM, BM); break;   \
-    case 128: HB_TG(128, AM, BM); break; \
-    default: HB_TG(256, AM, BM); break;  \
+  switch (BN) {
+    case 32: HB_TG(32); break;
+    case 64: HB_TG(64); break;
+    default: HB_TG(128); break;
   }
-  if (!a_mn && !b_mn) { HB_TG_BN(0, 0) }
-  else if (!a_mn && b_mn) { HB_TG_BN(0, 1) }
-  else if (a_mn && !b_mn) { HB_TG_BN(1, 0) }
-  else { HB_TG_BN(1, 1) }
-#undef HB_TG_BN
 #undef HB_TG
   HB_LAUNCH_OK();
   count_launch(1);

@@ -1,11 +1,11 @@
-// hb200 -- TMA halo load probe (verified on a B200; not on the product path yet).
+// hb200 -- TMA halo load probe (pins the halo kernels' tensor-map encoding; not on the product path).
 //
 // Next step for the halo convolutions (NOTES_NEXT.md item 4): replace the per-thread zero-filling cp.async gather of the
 // (TH+KH-1) x (TW+KW-1) input halo -- ~6 copies per thread, each with its own address and bounds predicate, the reason
 // conv_halo_kernel<32,32> is issue-bound -- by C/8 `cp.async.bulk.tensor.4d` box copies issued by ONE thread: box =
 // {8 channels, halo width, halo height, 1 frame} of the NHWC tensor, out-of-bounds rows / columns zero-filled by the TMA
 // unit (that is the conv padding), completion signalled on an mbarrier.  The box lands as [hy][hx][8 ch] = one 16-byte
-// vector per pixel, i.e. exactly one channel-chunk slab of the no-swizzle K-major operand layout the tcgen05 shared-
+// vector per pixel, i.e. exactly one channel-chunk slab of the no-swizzle K-major operand layout the wgmma shared-
 // memory descriptors address with LBO = slab stride (next 8 channels) and SBO = halo row pitch (next 8-pixel row group).
 //
 // This file only verifies the mechanism (driver entry point, tensor-map encoding, negative coordinates, expect_tx
@@ -13,11 +13,11 @@
 #include <cuda.h>
 
 #include "common.cuh"
-#include "umma.cuh"
+#include "wgmma.cuh"
 
 namespace hb200 {
 void count_launch(int n);
-using namespace umma;
+using namespace wg;
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
                                   const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,

@@ -267,7 +267,7 @@ def gn_bwd(g, act, y, stats, gamma, beta, dgamma, dbeta, dy, gz_out, batch, hw, 
 
 
 # ---- dense / rnn / misc -----------------------------------------------------------------------------------
-DENSE_TF32 = True  # dense layers on tcgen05 kind::tf32 (the reference's cuDNN-RNN precision); False -> fp32 SIMT
+DENSE_TF32 = True  # dense layers on wgmma tf32 (the reference's cuDNN-RNN precision); False -> fp32 SIMT
 
 
 def _tf32_ok(a, a_ms, a_ks, b, b_ks, b_ns, m, n, k):

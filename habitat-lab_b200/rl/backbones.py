@@ -2,7 +2,7 @@
 (resnet18 / resnet50 / resneXt50 / se_resnet50 / se_resneXt50 / se_resneXt101) with the reference's module names, so
 that `state_dict()` keys and shapes interchange with reference checkpoints.
 
-Only resnet18 has sm_100a kernels behind it today (rl/resnet_policy.py builds its own resnet18 holders and the conv
+Only resnet18 has sm_90a kernels behind it today (rl/resnet_policy.py builds its own resnet18 holders and the conv
 engine); the Bottleneck families are the SURVEY 8f-2 "next" row.  These holders exist so that the checkpoint contract
 of configs #3 / #4 is pinned now (tests/test_host_api.py checks them against the layouts recorded from the real
 reference in tests/golden/r50_objectnav.pt and rx50_imagenav.pt); they perform no computation."""

@@ -7,7 +7,7 @@ trainer / agent-access-manager read, and a state_dict with the reference's exact
 shapes (the torch.nn modules below are parameter holders + initialisers only; their forward is
 never called).  All arithmetic runs in libhb200.so:
 
-  forward  : prep (u8/f32 rollout rows -> pooled, normalised bf16 NHWC) -> tcgen05 conv stack with
+  forward  : prep (u8/f32 rollout rows -> pooled, normalised bf16 NHWC) -> wgmma conv stack with
              GroupNorm statistics fused in the epilogue -> fp32 linears / masked LSTM -> heads
   backward : hand-written, layer by layer, into one flat fp32 gradient buffer (no autograd)
 

@@ -1,4 +1,4 @@
-/* hb200.h -- C ABI of libhb200.so: the B200 (sm_100a) DD-PPO learner hot path that
+/* hb200.h -- C ABI of libhb200.so: the H100 (sm_90a) DD-PPO learner hot path that
  * sits below habitat-baselines' Python registry classes.
  *
  * The reference (facebookresearch/habitat-lab) has NO native boundary: every hot-path
@@ -17,8 +17,8 @@
  *    element format is fixed per argument): FORWARD values -- the pooled network input, conv outputs `y`, normalised
  *    activations, the packed forward weight images -- are IEEE fp16 (11-bit significand: what the reference's TF32
  *    cuDNN convolutions keep of their operands); GRADIENTS (g / dy / dx / gz / addend), the transposed (dgrad)
- *    weight images and the `*_bf16` twin outputs read by the weight-gradient kernels are bfloat16.  tcgen05
- *    kind::f16 needs both MMA operands in ONE format, so the forward kernels can write a second, bf16-rounded copy
+ *    weight images and the `*_bf16` twin outputs read by the weight-gradient kernels are bfloat16.  The
+ *    tensor core (wgmma) needs both MMA operands in ONE format, so the forward kernels can write a second, bf16-rounded copy
  *    of an activation (`out_bf16`, optional): the weight gradient dW = sum x * dy then multiplies bf16 x with bf16 dy.
  *    Rounding x there is harmless (a linear perturbation); rounding it in the FORWARD pass is not (it flips ReLU /
  *    max-pool decisions), which is why the forward copy is fp16.
@@ -164,7 +164,7 @@ int hb200_relu_bias_bwd(const hb200_bf16* g, const hb200_bf16* out, hb200_bf16* 
 int hb200_bf16_hwc_to_f32_chw(const hb200_bf16* x, float* out, int batch, int hw, int channels,
                               hb200_stream_t stream);
 
-/* ---- implicit-GEMM convolution on tcgen05 tensor cores -----------------------------------
+/* ---- implicit-GEMM convolution on the tensor cores (wgmma) --------------------------------
  * replaces nn.Conv2d forward / backward-data / backward-weight as dispatched by
  * HB/rl/ddppo/policy/resnet.py:15-34,207-219 and resnet_policy.py:224-234 (cuDNN today).
  *
@@ -189,7 +189,7 @@ int hb200_conv_bias_act_fwd(const hb200_bf16* x, const hb200_bf16* w_packed, con
 /* dy [B,Ho,Wo,Co] -> dx [B,Hi,Wi,Ci]; w_packed_t bf16 [Ci][kh*kw*Co padded] (transposed pack) */
 int hb200_conv_dgrad(const hb200_bf16* dy, const hb200_bf16* w_packed_t, const hb200_bf16* addend,
                      hb200_bf16* dx, const hb200_conv_shape* s, hb200_stream_t stream);
-/* dw_acc f32 [kh*kw*Ci][Co], ACCUMULATED with atomics (caller zeroes) */
+/* dw_acc f32 [kh*kw*Ci][Co], ACCUMULATED (+=; caller zeroes): per-split partials summed in a fixed order */
 int hb200_conv_wgrad(const hb200_bf16* x, const hb200_bf16* dy, float* dw_acc,
                      const hb200_conv_shape* s, hb200_stream_t stream);
 /* f32 OIHW [Co,Ci_real,kh,kw] -> bf16 [Co][(r,s,ci) padded] (ci_pad >= ci_real, zero filled),
@@ -211,7 +211,7 @@ int hb200_get_umma_layout(void);
 
 /* ---- "halo" convolutions: stride-1 k x k layers (k=3 pad 1; k=4 = the space-to-depth stem) ----------
  * Each CTA loads the input halo of a 16x8 output tile once and addresses every filter tap with a
- * shifted tcgen05 shared-memory descriptor (no im2col re-reads); persistent CTAs keep the weights
+ * shifted wgmma shared-memory descriptor (no im2col re-reads); persistent CTAs keep the weights
  * (forward/dgrad) or the accumulators (wgrad) resident.  Same reference ops as hb200_conv_* above.
  * wimg: hb200_pack_halo_weight image [taps][C/8][N][8] (mode 0 forward, 1 dgrad, 2 stem).
  * mode 0 forward (gn_stats optional) / 1 data gradient (addend optional). */
@@ -266,14 +266,14 @@ int hb200_conv_s2_dgrad(const hb200_bf16* dya, const hb200_bf16* dyb, const hb20
                         const hb200_bf16* addend, hb200_bf16* dx, int batch, int h, int w, int c, int na, int nb,
                         hb200_stream_t stream);
 
-/* dw_acc f32 [(r*k+s)*C + ci][N] accumulated with atomics (caller zeroes), like hb200_conv_wgrad */
+/* dw_acc f32 [(r*k+s)*C + ci][N] accumulated (+=; caller zeroes) in a fixed order, like hb200_conv_wgrad */
 int hb200_conv_halo_wgrad(const hb200_bf16* x, const hb200_bf16* dy, float* dw_acc, int batch, int h, int w,
                           int c, int n, int k, hb200_stream_t stream);
 /* stem accumulator [(a*4+b)*16 + (dy,dx,c)][Co] -> f32 OIHW [Co,Ci_real,7,7] */
 int hb200_unpack_stem_wgrad(const float* dw_acc, float* dw_oihw, int co, int ci_real, hb200_stream_t stream);
 
-/* raw tcgen05 GEMM probe: D[M,N] f32 = A[M,K] * B[N,K]^T (bf16, K-major both), M%128==0,
- * N%16==0 && N<=256, K%64==0.  layout: 0 = K-major no-swizzle interleaved core matrices,
+/* raw wgmma GEMM probe: D[M,N] f32 = A[M,K] * B[N,K]^T (bf16, or fp16 with flags 16 | 32: both operands share one
+ * format), M%128==0, N in {16, 32, 64, 128}, K%64==0.  layout: 0 = K-major no-swizzle interleaved core matrices,
  * 1 = K-major 128B swizzle, 2 = MN-major no-swizzle (then A is given as [K,M], B as [K,N]).
  * Used by the tests to pin the smem/instruction descriptor encodings on hardware. */
 int hb200_umma_gemm_probe(const hb200_bf16* a, const hb200_bf16* b, float* d, int m, int n, int k,
@@ -345,11 +345,11 @@ int hb200_gn_bwd_apply(const hb200_bf16* g, const hb200_bf16* act, const hb200_b
 int hb200_sgemm(const float* a, long long a_ms, long long a_ks, const float* b, long long b_ks,
                 long long b_ns, float* c, long long ldc, const float* bias, int m, int n, int k,
                 float alpha, int accumulate, int relu, hb200_stream_t stream);
-/* Same contract on the tensor cores: tcgen05 kind::tf32 (operands stay fp32 in memory, read as TF32 --
+/* Same contract on the tensor cores: wgmma .tf32 (operands stay fp32 in memory, read as TF32 --
  * the precision of the reference's cuDNN RNN path on CUDA -- fp32 accumulation).  Both operands must be
  * K-major (a_ks == 1 and b_ks == 1; transposed operands go through hb200_transpose_f32) with 16-byte
  * aligned rows (leading dimensions multiples of 4 floats).  Weight gradients
- * (accumulate != 0, long K) are split over K with fp32 atomics. */
+ * (accumulate != 0, long K) are split over K; the splits are summed in split order. */
 int hb200_tgemm(const float* a, long long a_ms, long long a_ks, const float* b, long long b_ks, long long b_ns,
                 float* c, long long ldc, const float* bias, int m, int n, int k, int accumulate, int relu,
                 hb200_stream_t stream);
@@ -463,7 +463,7 @@ int hb200_embed_fwd(const float* goal, const int64_t* prev_actions, const uint8_
                     const int32_t* frame_rows, const float* w_tgt, const float* b_tgt,
                     const float* emb_table, float* out, int ld, int col0, int batch,
                     hb200_stream_t stream);
-/* d_out f32 [B,ld]; d_w_tgt [32,3], d_b_tgt [32], d_emb [A+1,32] accumulated with atomics */
+/* d_out f32 [B,ld]; d_w_tgt [32,3], d_b_tgt [32], d_emb [A+1,32] accumulated (+=) in a fixed frame order */
 int hb200_embed_bwd(const float* goal, const int64_t* prev_actions, const uint8_t* masks,
                     const int32_t* frame_rows, const float* d_out, int ld, int col0, int batch,
                     int n_emb, float* d_w_tgt, float* d_b_tgt, float* d_emb,

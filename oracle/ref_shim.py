@@ -22,12 +22,12 @@ _REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 def _pick_root() -> str:
-    """/root/reference in the build container; on the GPU box (where it does not exist) the verbatim copy that
-    baseline/install_reference.py placed under baseline/_ref/ (git-ignored, shipped with the snapshot)."""
+    """The verbatim copy oracle/install_reference.py placed under oracle/_ref/ (git-ignored) when build() ran next to
+    a reference checkout, else the checkout itself."""
     env = os.environ.get("HB200_REFERENCE_ROOT")
     if env:
         return env
-    for cand in ("/root/reference", os.path.join(_REPO, "baseline", "_ref")):
+    for cand in (os.path.join(_REPO, "oracle", "_ref"), "/root/reference"):
         if os.path.isdir(os.path.join(cand, "habitat-baselines", "habitat_baselines")):
             return cand
     return "/root/reference"

@@ -280,6 +280,51 @@ def main():
                os.path.join(HERE, "rnn_lstm.pt"))
     print("rnn golden saved")
 
+    ppo_loss_case(R)
+
+
+def ppo_loss_case(R):
+    """PPO._update_from_batch's loss section with a linear actor-critic stand-in on seeded random tensors: the inputs
+    and the reference's metrics (tests/test_oracle.py::test_oracle_against_live_reference_ppo_loss)."""
+    import collections
+
+    torch.manual_seed(0)
+    B, A = 64, 4
+    feats = torch.randn(B, 512)
+
+    class FakeAC(torch.nn.Module):
+        def __init__(self):
+            super().__init__()
+            self.lin = torch.nn.Linear(512, A)
+            self.val = torch.nn.Linear(512, 1)
+
+        def evaluate_actions(self, obs, h, pa, m, actions, info):
+            dist = torch.distributions.Categorical(logits=self.lin(obs))
+            return self.val(obs), dist.log_prob(actions.squeeze(-1)).unsqueeze(-1), dist.entropy().unsqueeze(-1), h, {}
+
+        def policy_parameters(self):
+            return self.parameters()
+
+        def aux_loss_parameters(self):
+            return {}
+
+    ac = FakeAC()
+    ppo = R.PPO(ac, clip_param=0.2, ppo_epoch=1, num_mini_batch=1, value_loss_coef=0.5, entropy_coef=0.01, lr=0.0,
+                eps=1e-5, max_grad_norm=0.2, use_clipped_value_loss=True, use_normalized_advantage=False)
+    batch = dict(observations=feats, recurrent_hidden_states=None, prev_actions=None, masks=None,
+                 actions=torch.randint(0, A, (B, 1)), action_log_probs=torch.randn(B, 1) * 0.3 - 1.4,
+                 advantages=torch.randn(B, 1), value_preds=torch.randn(B, 1) * 0.3, returns=torch.randn(B, 1))
+    metrics = collections.defaultdict(list)
+    ppo._update_from_batch(batch, 0, None, metrics)
+    keys = ("value_loss", "action_loss", "dist_entropy", "value_pred_min", "value_pred_mean", "value_pred_max",
+            "prob_ratio_min", "prob_ratio_mean", "prob_ratio_max", "ppo_fraction_clipped")
+    out = {"metrics": {k: float(metrics[k][0]) for k in keys}, "feats": feats,
+           "lin_w": ac.lin.weight.detach().clone(), "lin_b": ac.lin.bias.detach().clone(),
+           "val_w": ac.val.weight.detach().clone(), "val_b": ac.val.bias.detach().clone(),
+           **{k: v for k, v in batch.items() if isinstance(v, torch.Tensor) and k != "observations"}}
+    torch.save(out, os.path.join(HERE, "ppo_loss_reference.pt"))
+    print("ppo_loss_reference", out["metrics"])
+
 
 if __name__ == "__main__":
     main()

@@ -1,4 +1,4 @@
-"""CPU: the reference arm of bench.py (`--impl reference`: the UNMODIFIED reference's CPU learner from baseline/_ref) prints exactly
+"""CPU: the reference arm of bench.py (`--impl reference`: the UNMODIFIED reference's CPU learner from oracle/_ref) prints exactly
 one JSON line on stdout with the keys the driver reads, whatever libraries print meanwhile."""
 import json
 import os

@@ -245,7 +245,7 @@ def test_ppo_loss_importance_coefficients(hb):
 
 
 # ---------------------------------------------------------------------------------------------
-# tcgen05 descriptor probe + convolutions
+# wgmma descriptor probe + convolutions
 # ---------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("layout", [0, 2])
 def test_umma_probe(hb, layout):
@@ -266,11 +266,9 @@ def test_umma_probe(hb, layout):
 @pytest.mark.parametrize("layout", [0, 1, 2])
 @pytest.mark.parametrize("a_f16,b_f16", [(True, True)])
 def test_umma_probe_operand_formats(hb, layout, a_f16, b_f16):
-    """kind::f16 with fp16 operands (the forward convolutions; gradients use bf16 x bf16, test_umma_probe).  Values
-    carry > 8 significant bits so a wrong format field (fp16 bits read as bf16) cannot pass.  MIXED fp16 x bf16
-    descriptors are deliberately not exercised: on B200 they raise an illegal-instruction fault that kills the CUDA
-    context (measured in round 2, profiles/r02_notes.md) -- the reason the weight-gradient kernels read a bf16 twin of
-    the activations instead."""
+    """fp16 x fp16 operands (the forward convolutions; gradients use bf16 x bf16, test_umma_probe).  Values carry > 8
+    significant bits so a wrong operand type (fp16 bits read as bf16) cannot pass.  The tensor core has no MIXED
+    fp16 x bf16 form -- the reason the weight-gradient kernels read a bf16 twin of the activations."""
     from habitat_lab_b200 import ops
 
     m, n, k = 256, 64, 192
@@ -303,7 +301,7 @@ CONV_CASES = [
     (2, 128, 128, 1, 8, 32, 8, 4, 0),     # SimpleCNN conv 1 (depth only), simple_cnn.py:84-96
     (2, 31, 31, 32, 32, 64, 4, 2, 0),     # SimpleCNN conv 2 (odd input, last row/col unused)
     (2, 14, 14, 64, 64, 32, 3, 1, 0),     # SimpleCNN conv 3 (no padding)
-    # the cases above have < 148 row tiles: the gather kernel slices the packed N tile (32-wide CTAs, the actor's
+    # the cases above have < 132 row tiles: the gather kernel slices the packed N tile (32-wide CTAs, the actor's
     # launch shape); these two keep the full-width tiles of the learner's 4096-frame minibatches covered
     (1200, 4, 4, 256, 256, 256, 3, 1, 1),
     (300, 8, 8, 64, 64, 128, 3, 2, 1),
@@ -804,7 +802,7 @@ def tgemm_feed(hb, request):
                                    # one row tile (the actor's batches): deterministic split-K through the workspace
                                    (64, 512, 2048), (64, 2048, 576), (64, 2048, 512), (3, 36, 260), (128, 512, 4096)])
 def test_tgemm_tf32(hb, tgemm_feed, M, N, K):
-    """tcgen05 kind::tf32 dense layers: forward (K-major x K-major), data gradient (K-major x N-major) and
+    """wgmma tf32 dense layers: forward (K-major x K-major), data gradient (K-major x N-major) and
     split-K weight gradient (M-major x N-major) vs fp64; tolerance = TF32 operand rounding (2^-11 relative)."""
     from habitat_lab_b200 import ops
 

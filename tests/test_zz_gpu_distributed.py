@@ -4,10 +4,9 @@ DDP cannot make: the reduced gradient equals the single-process mean of the rank
 RunningMeanAndVar all-reduce leaves identical running statistics on every rank, and `before_step` produces the same
 parameters a single process gets from the averaged gradient.
 
-Two processes are spawned, one GPU each, NCCL backend (what the bench runs): the test needs >= 2 visible GPUs
-(`gpurun --gpus 2 -- python -m pytest tests/test_zz_gpu_distributed.py`, result recorded in profiles/) and is SKIPPED
-on a 1-GPU box -- two processes time-slicing one GPU with persistent tcgen05 / cooperative kernels is not a
-configuration the path supports (round 2: it wedged the device for every later process on that box).  The file name
+Two processes are spawned, one GPU each, NCCL backend (what the bench runs): the test needs >= 2 visible GPUs and is
+SKIPPED on a 1-GPU machine -- two processes time-slicing one GPU with persistent / cooperative kernels is not a
+configuration the path supports.  The file name
 sorts last so that, whatever happens here, every other GPU test has already run.  bench.py asserts the same
 cross-rank equality after its timed steps at N = 2 / 4 / 8 (`cross_rank_equality` in the JSON line)."""
 import os

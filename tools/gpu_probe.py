@@ -1,15 +1,19 @@
-"""Runs on the GPU box: pins the tcgen05 descriptor encodings by running the raw GEMM probe for
-every shared-memory layout in its own process (a trap poisons the CUDA context) and writes the
-result table to gpurun_out/probe.json."""
+"""Pins the wgmma shared-memory descriptor encodings on the GPU by running the raw GEMM probe for every
+shared-memory layout and tile width in its own process, and writes the result table as JSON to the path given as the
+only argument (default: hb200_probe.json in the system temporary directory).
+
+    python tools/gpu_probe.py [OUT.json]
+"""
 import json
 import os
 import subprocess
 import sys
+import tempfile
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
-CASES = [(layout, n, k) for layout in (0, 1, 2) for (n, k) in ((32, 64), (64, 128), (256, 192), (128, 576))]
+CASES = [(layout, n, k) for layout in (0, 1, 2) for (n, k) in ((32, 64), (64, 128), (16, 192), (128, 576))]
 
 
 def one(layout, n, k):
@@ -50,6 +54,7 @@ if __name__ == "__main__":
         except subprocess.TimeoutExpired:
             out.append({"layout": layout, "n": n, "k": k, "error": "timeout"})
         print(out[-1], flush=True)
-    os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
-    with open(os.path.join(ROOT, "gpurun_out", "probe.json"), "w") as f:
+    path = sys.argv[1] if len(sys.argv) == 2 else os.path.join(tempfile.gettempdir(), "hb200_probe.json")
+    with open(path, "w") as f:
         json.dump(out, f, indent=1)
+    print("wrote", path)

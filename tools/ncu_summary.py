@@ -1,6 +1,5 @@
-"""Summarise .ncu-rep files (ncu --set full) into a small markdown/JSON table for profiles/:
-per launch: duration, DRAM bytes read+written (the `traffic` of bench.py's roofline), DRAM / L2 / tensor-pipe / issue
-utilisation, occupancy, registers."""
+"""Summarise .ncu-rep files (ncu --set full) into a small markdown/JSON table:
+per launch: duration, DRAM bytes read+written, DRAM / L2 / tensor-pipe / issue utilisation, occupancy, registers."""
 import csv
 import io
 import json

@@ -1,10 +1,15 @@
-"""Runs on the GPU box: how far is the REFERENCE's own CUDA path (cuDNN TF32 convolutions, torch defaults) from its
-fp32 CPU path?  Same minibatch as tests/golden/bench128.pt (T=128 x 8 envs = 1024 frames of 256x256 RGB-D), unmodified
-reference classes from baseline/_ref, per-tensor gradient cosine / norm ratio of device=cuda vs device=cpu.
-Writes gpurun_out/ref_cuda_precision.json -- the yardstick the hb200 precision bars are read against."""
+"""How far is the REFERENCE's own CUDA path (cuDNN TF32 convolutions, torch defaults) from its fp32 CPU path?  Same
+minibatch as tests/golden/bench128.pt (T=128 x 8 envs = 1024 frames of 256x256 RGB-D), unmodified reference classes from
+oracle/_ref, per-tensor gradient cosine / norm ratio of device=cuda vs device=cpu -- the yardstick the hb200 precision
+bars are read against.  Writes JSON to the path given as the second argument (default: hb200_ref_cuda_precision.json
+in the system temporary directory).
+
+    python tools/ref_cuda_precision.py [FIXTURE (default bench128) [OUT.json]]
+"""
 import json
 import os
 import sys
+import tempfile
 
 import numpy as np
 import torch
@@ -71,8 +76,10 @@ def main():
                     "median_cos_encoder": sorted(x[0] for x in enc)[len(enc) // 2],
                     "max_norm_dev_encoder": max(abs(x[1] - 1) for x in enc)}
         print(tag, json.dumps(out[tag])[:600])
-    os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
-    json.dump(out, open(os.path.join(ROOT, "gpurun_out", "ref_cuda_precision.json"), "w"), indent=1)
+    path = sys.argv[2] if len(sys.argv) > 2 else os.path.join(tempfile.gettempdir(), "hb200_ref_cuda_precision.json")
+    with open(path, "w") as f:
+        json.dump(out, f, indent=1)
+    print("wrote", path)
 
 
 if __name__ == "__main__":

@@ -146,9 +146,4 @@ __device__ __forceinline__ uint4 pack8a(const float (&f)[8]) {
   return u;
 }
 
-// 16-byte vector reduction to global memory (sm_90+): one L2 transaction for 4 floats
-__device__ __forceinline__ void red_add_v4(float* addr, float a, float b, float c, float d) {
-  asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(addr), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
-}
-
 }  // namespace hb200

@@ -1143,34 +1143,26 @@ __global__ void sensor_linear_fwd_kernel(const float* __restrict__ x, int in_dim
   }
 }
 // d_w[j, k] += sum_f d_out[f, col0 + j] feat_k ; d_b[j] += sum_f d_out[f, col0 + j]   (out_dim <= 64, nfeat <= 8)
+// Thread i owns accumulator i of [d_w (out_dim x nf) | d_b (out_dim)] and walks the frames of chunk blockIdx.y in
+// order; the per-chunk partials are added in order by reduce_partials (like embed_bwd: the same result every run).
 __global__ void sensor_linear_bwd_kernel(const float* __restrict__ x, int in_dim, const int32_t* __restrict__ rows,
                                          int B, int transform, const float* __restrict__ d_out, int ld, int col0,
-                                         int out_dim, float* __restrict__ d_w, float* __restrict__ d_b) {
-  __shared__ float acc[64 * 9];
-  for (int i = threadIdx.x; i < out_dim * 9; i += blockDim.x) acc[i] = 0.f;
-  __syncthreads();
-  const long long total = (long long)B * out_dim;
-  int nf = 0;
-  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total;
-       i += (long long)gridDim.x * blockDim.x) {
-    const int f = (int)(i / out_dim), j = (int)(i - (long long)f * out_dim);
-    float ft[8];
-    nf = sensor_features(x + (size_t)rows[f] * in_dim, in_dim, transform, ft);
+                                         int out_dim, int nf, float* __restrict__ parts) {
+  const int nacc = out_dim * (nf + 1);
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= nacc) return;
+  const bool bias = i >= out_dim * nf;
+  const int j = bias ? i - out_dim * nf : i / nf, k = bias ? 0 : i - j * nf;
+  const int f0 = blockIdx.y * kEmbedFrames, f1 = min(B, f0 + kEmbedFrames);
+  float v = 0.f;
+  for (int f = f0; f < f1; ++f) {
     const float d = d_out[(size_t)f * ld + col0 + j];
-    for (int k = 0; k < nf; ++k) atomicAdd(&acc[j * 9 + k], d * ft[k]);
-    atomicAdd(&acc[j * 9 + 8], d);
+    if (bias) { v += d; continue; }
+    float ft[8];
+    sensor_features(x + (size_t)rows[f] * in_dim, in_dim, transform, ft);
+    v = fmaf(d, ft[k], v);
   }
-  __syncthreads();
-  float ft0[8];
-  const float zero[3] = {0.f, 0.f, 0.f};
-  nf = sensor_features(zero, in_dim, transform, ft0);   // feature count only
-  for (int i = threadIdx.x; i < out_dim * 9; i += blockDim.x) {
-    const int j = i / 9, k = i - j * 9;
-    const float v = acc[i];
-    if (v == 0.f) continue;
-    if (k == 8) atomicAdd(&d_b[j], v);
-    else if (k < nf) atomicAdd(&d_w[j * nf + k], v);
-  }
+  parts[(size_t)blockIdx.y * nacc + i] = v;
 }
 // out[f, col0 + j] = table[index_f, j]; index from an int64 tensor through rows (objectgoal) or, with masks,
 // masks[f] ? idx[f] + 1 : 0 (the previous-action embedding with its "start" token, resnet_policy.py:747-757)
@@ -1188,17 +1180,24 @@ __global__ void index_embed_fwd_kernel(const int64_t* __restrict__ idx, const in
     out[(size_t)f * ld + col0 + j] = (k >= 0 && k < n_rows_table) ? table[k * width + j] : __int_as_float(0x7fc00000);
   }
 }
+// Thread i owns d_table element i (row i / width) and adds the frames of chunk blockIdx.y that index its row, in
+// frame order; the per-chunk partials are added in order by reduce_partials.  Out-of-range indices add nothing.
 __global__ void index_embed_bwd_kernel(const int64_t* __restrict__ idx, const int32_t* __restrict__ rows,
                                        const uint8_t* __restrict__ masks, int B, int n_rows_table, int width,
-                                       const float* __restrict__ d_out, int ld, int col0, float* __restrict__ d_table) {
-  const long long total = (long long)B * width;
-  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total;
-       i += (long long)gridDim.x * blockDim.x) {
-    const int f = (int)(i / width), j = (int)(i - (long long)f * width);
+                                       const float* __restrict__ d_out, int ld, int col0, float* __restrict__ parts) {
+  const long long nacc = (long long)n_rows_table * width;
+  const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  if (i >= nacc) return;
+  const long long row = i / width;
+  const int j = (int)(i - row * width);
+  const int f0 = blockIdx.y * kEmbedFrames, f1 = min(B, f0 + kEmbedFrames);
+  float v = 0.f;
+  for (int f = f0; f < f1; ++f) {
     long long k = idx[rows ? (size_t)rows[f] : (size_t)f];
     if (masks) k = masks[f] ? k + 1 : 0;
-    if (k >= 0 && k < n_rows_table) atomicAdd(&d_table[k * width + j], d_out[(size_t)f * ld + col0 + j]);
+    if (k == row) v += d_out[(size_t)f * ld + col0 + j];
   }
+  parts[(size_t)blockIdx.y * nacc + i] = v;
 }
 
 // ---- generic visual input prep: any mix of u8 / f32 / i32 HWC sensors, any H x W ----------------------------------
@@ -1481,9 +1480,10 @@ __global__ void prep_plain_kernel(const uint8_t* __restrict__ rgb, const float* 
   }
 }
 // backward of (conv + bias) -> ReLU: dy = g * (out > 0); dbias[c] += sum dy   (out = post-ReLU activation)
+// Each block writes its per-channel partial to parts[blockIdx.x][C]; reduce_partials adds them in block order.
 __global__ void __launch_bounds__(256)
 relu_bias_bwd_kernel(const grad_t* __restrict__ g, const act_t* __restrict__ out, int use_mask,
-                     grad_t* __restrict__ dy, float* __restrict__ dbias, long long npix, int C) {
+                     grad_t* __restrict__ dy, float* __restrict__ parts, long long npix, int C) {
   __shared__ float sacc[256][9];
   const int cv = C >> 3;
   const int vec = threadIdx.x % cv, pl = threadIdx.x / cv, npl = blockDim.x / cv;
@@ -1507,7 +1507,7 @@ relu_bias_bwd_kernel(const grad_t* __restrict__ g, const act_t* __restrict__ out
   for (int c = threadIdx.x; c < C; c += blockDim.x) {
     float t = 0.f;
     for (int q = 0; q < npl; ++q) t += sacc[q * cv + (c >> 3)][c & 7];
-    atomicAdd(&dbias[c], t);
+    parts[(size_t)blockIdx.x * C + c] = t;
   }
 }
 // bf16 NHWC [B,hw,C] -> f32 [B, C*hw] flattened in (c,h,w) order (nn.Flatten of the NCHW map)
@@ -1876,13 +1876,22 @@ extern "C" int hb200_sensor_linear_bwd(const float* x, int in_dim, const int32_t
                                        hb200_stream_t stream) {
   HB_CHECK_ARG(x && frame_rows && d_out && d_w && d_b && batch > 0 && in_dim >= 1 && in_dim <= 8, "sensor_linear_bwd: bad args");
   HB_CHECK_ARG(transform >= 0 && transform <= 3 && out_dim >= 1 && out_dim <= 64, "sensor_linear_bwd: bad transform / width");
-  int grid = grid_for((long long)batch * out_dim, 256);
-  if (grid > kNumSMs) grid = kNumSMs;
-  sensor_linear_bwd_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(x, in_dim, frame_rows, batch, transform, d_out, ld,
-                                                                   col0, out_dim, d_w, d_b);
+  const int nf = transform == 1 ? 3 : (transform == 2 ? 4 : (transform == 3 ? 2 : in_dim));   // sensor_features
+  const int nacc = out_dim * (nf + 1), nparts = cdiv(batch, kEmbedFrames);
+  HB_CHECK_ARG(nparts <= 65535, "sensor_linear_bwd: batch %d exceeds %d frames", batch, 65535 * kEmbedFrames);
+  cudaStream_t st = (cudaStream_t)stream;
+  float* parts = nullptr;
+  int* tickets = nullptr;
+  int rc = stream_workspace(st, (size_t)(nparts + kReduceChunks) * nacc, 0, &parts, &tickets);
+  if (rc) return rc;
+  float* tmp = parts + (size_t)nparts * nacc;
+  sensor_linear_bwd_kernel<<<dim3(cdiv(nacc, 128), nparts), 128, 0, st>>>(x, in_dim, frame_rows, batch, transform, d_out,
+                                                                          ld, col0, out_dim, nf, parts);
   HB_LAUNCH_OK();
   count_launch(1);
-  return HB200_OK;
+  rc = reduce_partials(parts, nparts, nacc, (long long)out_dim * nf, d_w, tmp, st);
+  if (!rc) rc = reduce_partials(parts + (size_t)out_dim * nf, nparts, nacc, out_dim, d_b, tmp, st);
+  return rc;
 }
 
 extern "C" int hb200_index_embed_fwd(const int64_t* idx, const int32_t* frame_rows, const uint8_t* masks, int batch,
@@ -1900,11 +1909,19 @@ extern "C" int hb200_index_embed_bwd(const int64_t* idx, const int32_t* frame_ro
                                      int table_rows, int width, const float* d_out, int ld, int col0, float* d_table,
                                      hb200_stream_t stream) {
   HB_CHECK_ARG(idx && d_out && d_table && batch > 0 && table_rows > 0 && width > 0, "index_embed_bwd: bad args");
-  index_embed_bwd_kernel<<<grid_for((long long)batch * width, 256), 256, 0, (cudaStream_t)stream>>>(
-      idx, frame_rows, masks, batch, table_rows, width, d_out, ld, col0, d_table);
+  const long long nacc = (long long)table_rows * width;
+  const int nparts = cdiv(batch, kEmbedFrames);
+  HB_CHECK_ARG(nparts <= 65535, "index_embed_bwd: batch %d exceeds %d frames", batch, 65535 * kEmbedFrames);
+  cudaStream_t st = (cudaStream_t)stream;
+  float* parts = nullptr;
+  int* tickets = nullptr;
+  const int rc = stream_workspace(st, (size_t)(nparts + kReduceChunks) * nacc, 0, &parts, &tickets);
+  if (rc) return rc;
+  index_embed_bwd_kernel<<<dim3(cdiv(nacc, 128), nparts), 128, 0, st>>>(idx, frame_rows, masks, batch, table_rows, width,
+                                                                        d_out, ld, col0, parts);
   HB_LAUNCH_OK();
   count_launch(1);
-  return HB200_OK;
+  return reduce_partials(parts, nparts, nacc, nacc, d_table, parts + (size_t)nparts * nacc, st);
 }
 
 extern "C" int hb200_prep_generic(const void* const* h_srcs, const int* h_dtypes, const int* h_channels,
@@ -2152,11 +2169,16 @@ extern "C" int hb200_relu_bias_bwd(const hb200_bf16* g, const hb200_bf16* out, h
   int grid = (int)((npix + 255) / 256);
   if (grid > kNumSMs * 8) grid = kNumSMs * 8;
   if (grid < 1) grid = 1;
-  relu_bias_bwd_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>((const grad_t*)g, (const act_t*)out,
-                                                               out != nullptr, (grad_t*)dy, dbias, npix, channels);
+  cudaStream_t st = (cudaStream_t)stream;
+  float* parts = nullptr;
+  int* tickets = nullptr;
+  const int rc = stream_workspace(st, (size_t)(grid + kReduceChunks) * channels, 0, &parts, &tickets);
+  if (rc) return rc;
+  relu_bias_bwd_kernel<<<grid, 256, 0, st>>>((const grad_t*)g, (const act_t*)out, out != nullptr, (grad_t*)dy, parts,
+                                             npix, channels);
   HB_LAUNCH_OK();
   count_launch(1);
-  return HB200_OK;
+  return reduce_partials(parts, grid, channels, channels, dbias, parts + (size_t)grid * channels, st);
 }
 extern "C" int hb200_bf16_hwc_to_f32_chw(const hb200_bf16* x, float* out, int batch, int hw, int channels,
                                          hb200_stream_t stream) {

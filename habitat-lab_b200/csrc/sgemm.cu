@@ -66,7 +66,7 @@ __global__ void __launch_bounds__(256)
 sgemm_kernel(const float* __restrict__ a, long long a_ms, long long a_ks, const float* __restrict__ b,
              long long b_ks, long long b_ns, float* __restrict__ c, long long ldc,
              const float* __restrict__ bias, int M, int N, int K, float alpha, int accumulate, int relu,
-             int k_per_split) {
+             int k_per_split, float* __restrict__ ws) {
   __shared__ __align__(16) float As[BK][BM + 4];
   __shared__ __align__(16) float Bs[BK][BN + 4];
   const int m0 = blockIdx.y * BM, n0 = blockIdx.x * BN;
@@ -108,18 +108,28 @@ sgemm_kernel(const float* __restrict__ a, long long a_ms, long long a_ks, const 
       const int n = n0 + (j < 4 ? tx * 4 + j : 64 + tx * 4 + (j - 4));
       if (n >= N) continue;
       float v = alpha * acc[i][j];
-      float* dst = c + (long long)m * ldc + n;
-      if (gridDim.z > 1) {  // split-K: partial sums meet in a pre-zeroed (or accumulated-into) C
-        if (bias && blockIdx.z == 0) v += bias[n];
-        atomicAdd(dst, v);
+      if (gridDim.z > 1) {  // split-K: this split's partial, summed in split order by sgemm_split_sum_kernel
+        ws[((size_t)blockIdx.z * M + m) * N + n] = v;
         continue;
       }
+      float* dst = c + (long long)m * ldc + n;
       if (bias) v += bias[n];
       if (accumulate) v += *dst;
       if (relu) v = fmaxf(v, 0.f);
       *dst = v;
     }
   }
+}
+// C[m, n] += bias[n] + sum over z = 0 .. splits-1 of ws[z, m, n], always in that order (run-to-run identical)
+__global__ void sgemm_split_sum_kernel(const float* __restrict__ ws, int splits, float* __restrict__ c, long long ldc,
+                                       const float* __restrict__ bias, int M, int N) {
+  const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  if (i >= (long long)M * N) return;
+  const int m = (int)(i / N), n = (int)(i - (long long)m * N);
+  float v = ws[i];
+  for (int z = 1; z < splits; ++z) v += ws[(size_t)z * M * N + i];
+  if (bias) v += bias[n];
+  c[(long long)m * ldc + n] += v;
 }
 }  // namespace hb200
 
@@ -130,7 +140,8 @@ extern "C" int hb200_sgemm(const float* a, long long a_ms, long long a_ks, const
                            float alpha, int accumulate, int relu, hb200_stream_t stream) {
   HB_CHECK_ARG(a && b && c && m > 0 && n > 0 && k > 0, "sgemm: bad args");
   // split-K when the output tile grid cannot fill the GPU and the reduction is long (weight gradients:
-  // K = frames).  Needs C to hold the value to accumulate into -> only in accumulate mode without ReLU.
+  // K = frames).  Needs C to hold the value to accumulate into -> only in accumulate mode without ReLU.  The splits'
+  // partials go to the stream's workspace and are added in split order (no float atomics: same result every run).
   int splits = 1;
   {
     const long long tiles = (long long)cdiv(n, BN) * cdiv(m, BM);
@@ -146,8 +157,15 @@ extern "C" int hb200_sgemm(const float* a, long long a_ms, long long a_ks, const
   const int bm = (b_ns == 1) ? 0 : (b_ks == 1 ? 1 : 2);
   dim3 grid(cdiv(n, BN), cdiv(m, BM), splits);
   cudaStream_t st = (cudaStream_t)stream;
+  float* ws = nullptr;
+  if (splits > 1) {
+    int* tickets = nullptr;
+    const int rc = stream_workspace(st, (size_t)splits * m * n, 0, &ws, &tickets);
+    if (rc) return rc;
+  }
 #define HB_SG(AM, BMO) \
-  sgemm_kernel<AM, BMO><<<grid, 256, 0, st>>>(a, a_ms, a_ks, b, b_ks, b_ns, c, ldc, bias, m, n, k, alpha, accumulate, relu, k_per_split)
+  sgemm_kernel<AM, BMO><<<grid, 256, 0, st>>>(a, a_ms, a_ks, b, b_ks, b_ns, c, ldc, bias, m, n, k, alpha, accumulate, relu, \
+                                              k_per_split, ws)
   switch (am * 3 + bm) {
     case 0: HB_SG(0, 0); break;
     case 1: HB_SG(0, 1); break;
@@ -162,5 +180,10 @@ extern "C" int hb200_sgemm(const float* a, long long a_ms, long long a_ks, const
 #undef HB_SG
   HB_LAUNCH_OK();
   count_launch(1);
+  if (splits > 1) {
+    sgemm_split_sum_kernel<<<cdiv((long long)m * n, 256), 256, 0, st>>>(ws, splits, c, ldc, bias, m, n);
+    HB_LAUNCH_OK();
+    count_launch(1);
+  }
   return HB200_OK;
 }

@@ -475,7 +475,8 @@ int hb200_embed_bwd(const float* goal, const int64_t* prev_actions, const uint8_
  *            1 2-D polar pointgoal (r, cos(-t), sin(-t)) (:662-673), 2 3-D polar (:674-691),
  *            3 angle -> (cos, sin) (compass :718-728, heading :703-712).
  * out[f, col0 + j] = b[j] + sum_k w[j, k] feat_k  (w f32 [out_dim, n_feat], nn.Linear layout; out_dim <= 64);
- * w == NULL copies the features themselves (fuse keys).  _bwd accumulates d_w / d_b with atomics. */
+ * w == NULL copies the features themselves (fuse keys).  _bwd adds to d_w / d_b; frames are summed in a fixed order
+ * (per-chunk partials, then reduce_partials), so the result is the same every run. */
 int hb200_sensor_linear_fwd(const float* x, int in_dim, const int32_t* frame_rows, int batch, int transform,
                             const float* w, const float* b, float* out, int ld, int col0, int out_dim,
                             hb200_stream_t stream);

@@ -67,12 +67,16 @@ struct ConvArgs {
 template <int BN, int MODE, int LAYOUT, int NST = kStages>
 __global__ void __launch_bounds__(128) conv_igemm_kernel(const ConvArgs a) {
   extern __shared__ __align__(16) uint8_t smem_raw[];
-  __shared__ float stage_buf[kStageFloats];
   constexpr uint32_t kABytes = kTileM * kChunkK * 2;
   constexpr uint32_t kBBytes = BN * kChunkK * 2;
   constexpr uint32_t kStageBytes = kABytes + kBBytes;
   static_assert(BN <= kMaxBN, "conv: N tile");
+  static_assert(NST * kStageBytes >= kStageFloats * sizeof(float), "conv: epilogue transpose buffer");
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
+  // the epilogue's transpose buffer reuses the operand ring: every load and MMA of the tile has completed by then.  A
+  // separate 17 KB buffer would put a CTA just over half of the SM's shared memory (one CTA per SM instead of two, and
+  // no second CTA's MMAs to run under this one's epilogue).
+  float* const stage_buf = reinterpret_cast<float*>(smem_raw + (smem_base - smem_u32(smem_raw)));
 
   const int tid = threadIdx.x, lane = tid & 31;
   const int n0 = blockIdx.y * BN;
@@ -258,7 +262,7 @@ __global__ void __launch_bounds__(128) conv_igemm_kernel(const ConvArgs a) {
     }
     cp_async_commit();
   }
-  wgmma_wait<0>();
+  wgmma_wait<0>();   // (also: the ring is no longer read, stage_buf may overwrite it)
   acc_fence(acc_t);
 
   // ---- epilogue: registers -> (stats | + addend) -> fp16 / bf16 NHWC ----

@@ -1020,13 +1020,18 @@ conv_halo_sw_kernel(const HaloArgs a, const __grid_constant__ CUtensorMap tmap) 
 // conv_halo_tma_kernel runs load -> MMA -> epilogue of consecutive tiles from one program order: with a single halo
 // stage the TMA latency of tile it+1 is exposed after every tile, and only a second CTA of the SM hides it.  Here the
 // loads run in their own warp and meet the consumers only at mbarriers:
-//   warp 4 (one lane)  producer: halo stage ring, NS deep (as many as fit next to the resident weights)
-//   warps 0-3          one warpgroup: waits full[stage], issues the tile's MMAs, releases the stage (empty[stage]) as
-//                      soon as they complete, then GroupNorm sums / addend / pack / store while the producer loads ahead
+//   warp 8 (one lane)  producer: halo stage ring, NS deep (as many as fit next to the resident weights)
+//   warps 0-3, 4-7     two consumer warpgroups; tile `it` of the CTA goes to warpgroup it & 1.  Each waits full[stage],
+//                      issues the tile's MMAs, releases the stage (empty[stage]) as soon as they complete, then runs the
+//                      GroupNorm sums / addend / pack / store while the other warpgroup's MMAs run on the next tile
+// The accumulator lives in registers, so one warpgroup cannot overlap its own epilogue with MMAs: the second one is what
+// keeps the tensor core busy.  Each warpgroup transposes through its own stage buffer (dynamic shared memory, after the
+// halo ring) under its own named barrier (1 + warpgroup).
 // SW: stage the halo as KW pre-shifted copies of whole pixel rows in the swizzled K-major layout (conv_halo_sw_kernel)
 // instead of 16-byte channel slabs: aligned operand reads for the MMAs at KW times the TMA bytes
+constexpr int kHaloWsThreads = 288;
 template <int C, int N, int KH, int KW, int PAD, int MODE, int NS, bool SW = false>
-__global__ void __launch_bounds__(160)
+__global__ void __launch_bounds__(kHaloWsThreads)
 conv_halo_ws_kernel(const HaloArgs a, const __grid_constant__ CUtensorMap tmap) {
   using Cfg = HaloCfg<C, N, KH, KW, PAD>;
   constexpr int CJ = Cfg::CJ, HH = Cfg::HH, HWD = Cfg::HWD;
@@ -1037,11 +1042,11 @@ conv_halo_ws_kernel(const HaloArgs a, const __grid_constant__ CUtensorMap tmap) 
   static_assert(!SW || RB == 64 || RB == 128, "swizzled halo copies: 32 or 64 channels");
   extern __shared__ __align__(16) uint8_t smem_raw[];
   __shared__ __align__(8) uint64_t full_bar[NS], empty_bar[NS];
-  __shared__ float stage_buf[kStageFloats];
   const uint32_t sbase = (smem_u32(smem_raw) + 1023u) & ~1023u;   // swizzle atoms are 1024-byte aligned
   const uint32_t s_w = sbase;
   const uint32_t s_halo0 = s_w + Cfg::W_BYTES;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  float* const stage_bufs = reinterpret_cast<float*>(smem_raw + (s_halo0 + NS * STAGE - smem_u32(smem_raw)));
   if (tid == 0) {
 #pragma unroll
     for (int i = 0; i < NS; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 1); }
@@ -1060,7 +1065,7 @@ conv_halo_ws_kernel(const HaloArgs a, const __grid_constant__ CUtensorMap tmap) 
   const int my_n = first < a.ntiles ? (a.ntiles - first + stride - 1) / stride : 0;
   const CUtensorMap* const tmap_p = &tmap;   // param-space address, taken in the kernel body
 
-  if (warp == 4) {
+  if (warp == 8) {
     if (lane == 0) {
       for (int it = 0; it < my_n; ++it) {
         const int st = it % NS;
@@ -1087,9 +1092,11 @@ conv_halo_ws_kernel(const HaloArgs a, const __grid_constant__ CUtensorMap tmap) 
   } else {
     // forward: fp16 input halo x fp16 weight image; dgrad: bf16 gradients x bf16 flipped / transposed image
     constexpr int kT = MODE == 0 ? kF16 : kBF16;
-    const int py = tid >> 3, px = tid & 7;
+    const int wgi = warp >> 2, t = tid & 127;
+    const int py = t >> 3, px = t & 7;
+    float* const stage_buf = stage_bufs + wgi * kStageFloats;
     float acc_t[N];
-    for (int it = 0; it < my_n; ++it) {
+    for (int it = wgi; it < my_n; it += 2) {
       const int st = it % NS;
       const int tile = first + it * stride;
       const int b = tile / tiles_per_img, r = tile - b * tiles_per_img;
@@ -1113,12 +1120,12 @@ conv_halo_ws_kernel(const HaloArgs a, const __grid_constant__ CUtensorMap tmap) 
       wgmma_commit();
       wgmma_wait<0>();
       acc_fence(acc_t);
-      if (tid == 0) mbar_arrive(&empty_bar[st]);   // the halo stage is free: the producer may refill it
+      if (t == 0) mbar_arrive(&empty_bar[st]);   // the halo stage is free: the producer may refill it
       const size_t pix = ((size_t)b * a.H + oh0 + py) * a.W + ow0 + px;
 #pragma unroll
       for (int col0 = 0; col0 < N; col0 += 32) {
         float acc_[32];
-        acc_row32(acc_t, col0, stage_buf, acc_);
+        acc_row32(acc_t, col0, stage_buf, acc_, 1 + wgi);
         if (MODE == 0 && a.stats != nullptr)
           halo_gn_stats_chunk(acc_, lane, N / a.gn_groups, a.stats + (size_t)b * a.gn_groups * 2, col0);
         const size_t o = pix * N + col0;
@@ -1259,23 +1266,24 @@ static int launch_halo_ws(const HaloArgs& a, cudaStream_t st) {
   }
   constexpr size_t slab = (size_t)((Cfg::HH * Cfg::HWD * 16 + 127) / 128 * 128);
   const size_t stage = SW ? (size_t)KW * Cfg::HH * 8 * C * 2 : Cfg::CJ * slab;
-  const size_t smem = Cfg::W_BYTES + (size_t)NS * stage + 1024;
+  // weights | NS halo stages | one transpose stage buffer per consumer warpgroup (+ 1024 for the alignment of the base)
+  const size_t smem = Cfg::W_BYTES + (size_t)NS * stage + 2 * kStageFloats * sizeof(float) + 1024;
   auto kern = conv_halo_ws_kernel<C, N, KH, KW, PAD, MODE, NS, SW>;
   static int grid_cache = 0;
   if (grid_cache == 0) {
     HB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    // resident CTAs per SM from the static limits (registers of 160 threads, shared memory)
+    // resident CTAs per SM from the static limits (registers of 288 threads, shared memory)
     cudaFuncAttributes fa;
     HB_CUDA(cudaFuncGetAttributes(&fa, (const void*)kern));
     const int regs = fa.numRegs > 0 ? fa.numRegs : 128;
-    int per_sm = 65536 / (((regs + 7) / 8 * 8) * 160);
+    int per_sm = 65536 / (((regs + 7) / 8 * 8) * kHaloWsThreads);
     const int by_smem = (int)((227 * 1024) / (smem + fa.sharedSizeBytes + 1024));
     if (by_smem < per_sm) per_sm = by_smem;
     if (per_sm < 1) per_sm = 1;
     grid_cache = kNumSMs * per_sm;
   }
   const int grid = grid_cache < a.ntiles ? grid_cache : a.ntiles;
-  kern<<<grid, 160, smem, st>>>(a, tmap);
+  kern<<<grid, kHaloWsThreads, smem, st>>>(a, tmap);
   HB_LAUNCH_OK();
   count_launch(1);
   return HB200_OK;
@@ -1503,10 +1511,10 @@ extern "C" int hb200_conv_halo(const hb200_bf16* x, const hb200_bf16* wimg, hb20
   // 2 / 3 / 4 / 5 force swizzled copies / warp-specialised slabs / warp-specialised swizzled / plain slabs everywhere.
   if (g_halo_tma == 1 && k == 3 && c == 64)
     return mode == 0 ? launch_halo_ws<64, 64, 3, 3, 1, 0, 2, true>(a, st) : launch_halo_ws<64, 64, 3, 3, 1, 1, 2, true>(a, st);
-  if (g_halo_tma == 1 && k == 3 && c == 32)   // 3 stages each: several CTAs per SM
-    return mode == 0 ? launch_halo_ws<32, 32, 3, 3, 1, 0, 3, true>(a, st) : launch_halo_ws<32, 32, 3, 3, 1, 1, 3, true>(a, st);
+  if (g_halo_tma == 1 && k == 3 && c == 32)   // one CTA per SM: 18 KB of weights, 6 halo stages, 2 transpose buffers
+    return mode == 0 ? launch_halo_ws<32, 32, 3, 3, 1, 0, 6, true>(a, st) : launch_halo_ws<32, 32, 3, 3, 1, 1, 6, true>(a, st);
   if (g_halo_tma == 1 && k == 4 && mode == 0) return launch_halo_ws<16, 32, 4, 4, 2, 0, 6>(a, st);
-  if (g_halo_tma == 6 && k == 3 && c == 32)   // experiment: 2 stages, more CTAs per SM
+  if (g_halo_tma == 6 && k == 3 && c == 32)   // experiment: 2 stages, two CTAs per SM
     return mode == 0 ? launch_halo_ws<32, 32, 3, 3, 1, 0, 2, true>(a, st) : launch_halo_ws<32, 32, 3, 3, 1, 1, 2, true>(a, st);
   if (g_halo_tma == 4 && k == 3 && c == 32)
     return mode == 0 ? launch_halo_ws<32, 32, 3, 3, 1, 0, 3, true>(a, st) : launch_halo_ws<32, 32, 3, 3, 1, 1, 3, true>(a, st);

@@ -206,17 +206,19 @@ __device__ __forceinline__ void mma128(float (&acc)[N], uint64_t da, uint32_t a_
   Wgmma<N, T>::template mma<TA, TB>(*reinterpret_cast<float(*)[N / 2]>(&acc[N / 2]), desc_add(da, a_hi), db, accum);
 }
 
-// barrier over the 128 threads of warpgroup 0 only (other warps of the CTA may be busy elsewhere)
-__device__ __forceinline__ void wg_bar_sync() { asm volatile("bar.sync 1, 128;" ::: "memory"); }
+// named barrier `id` (1, 2, ...; 0 is __syncthreads) over the 128 threads of one warpgroup only (other warps of the CTA
+// may be busy elsewhere).  Kernels with two consumer warpgroups give each its own id.
+__device__ __forceinline__ void wg_bar_sync(int id) { asm volatile("bar.sync %0, 128;" ::"r"(id) : "memory"); }
 
 constexpr int kStagePitch = 33;   // floats per staged row: conflict-free row-per-thread reads
 constexpr int kStageFloats = 128 * kStagePitch;
 // columns [col0, col0 + 32) of tile row t (t = thread of the warpgroup) -> r.  `stage` holds kStageFloats floats of
-// shared memory.  All 128 threads call it with the same compile-time col0 (the caller's loop is unrolled).
+// shared memory, private to the calling warpgroup, and `bar` is that warpgroup's named barrier.  All 128 threads call it
+// with the same compile-time col0 (the caller's loop is unrolled).
 template <int N>
-__device__ __forceinline__ void acc_row32(const float (&acc)[N], int col0, float* stage, float (&r)[32]) {
+__device__ __forceinline__ void acc_row32(const float (&acc)[N], int col0, float* stage, float (&r)[32], int bar = 1) {
   const int t = threadIdx.x & 127, w = t >> 5, l = t & 31;
-  wg_bar_sync();   // the previous slice has been read
+  wg_bar_sync(bar);   // the previous slice has been read
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
 #pragma unroll
@@ -229,7 +231,7 @@ __device__ __forceinline__ void acc_row32(const float (&acc)[N], int col0, float
       stage[(row + 8) * kStagePitch + col + 1] = acc[idx + 3];
     }
   }
-  wg_bar_sync();
+  wg_bar_sync(bar);
 #pragma unroll
   for (int j = 0; j < 32; ++j) r[j] = stage[t * kStagePitch + j];
 }

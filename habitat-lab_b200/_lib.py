@@ -77,6 +77,8 @@ SIGNATURES = {
     "hb200_gn_bwd_reduce": ("i", "ppppppppp" + "iiii" + "f" + "i" + "p"),
     "hb200_gn_bwd_apply": ("i", "ppppppppp" + "iiii" + "f" + "i" + "p"),
     "hb200_gn_bwd": ("i", "pppppppppp" + "iiii" + "f" + "i" + "p"),
+    "hb200_gn_se_residual_relu": ("i", "pppppppp" + "pppp" + "ppppp" + "iiiii" + "f" + "p"),
+    "hb200_gn_se_bwd": ("i", "pppppppppp" + "pppppp" + "iiiii" + "f" + "p"),
     "hb200_tma_halo_probe": ("i", "pp" + "iiiiiiiiii" + "p"),
     "hb200_gn_relu_maxpool_bwd_supported": ("i", "iiii"),
     "hb200_gn_relu_maxpool_bwd": ("i", "ppppppppp" + "iiiii" + "f" + "p"),

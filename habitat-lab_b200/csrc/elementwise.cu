@@ -1592,6 +1592,366 @@ static int gn_affine_grads_reduce(const float* part_g, const float* part_b, int 
   return reduce_partials(part_g, B, C, C, dgamma, tmp, st);
 }
 
+// ---- squeeze-excite block output (SEBottleneck, resnet.py:92-110, 155-180) ------------------------------------------
+//   z = GN(y),  p = mean_hw(z),  h = relu(W1 p + b1),  s = sigmoid(W2 h + b2),  o = relu(s * z + r)
+// p needs only per-channel sums of y: p = zc * mean_hw(y) + zd with zc = rstd * gamma, zd = beta - mu * zc.  In the
+// backward, with gz = g * [o > 0], every per-frame quantity follows from three per-channel sums (sum gz, sum gz*y,
+// sum y): ds = zc * sum(gz*y) + zd * sum(gz), a = ds * s * (1 - s), dh = (W2^T a) * [h > 0], dp = W1^T dh, and the
+// GroupNorm backward runs on dz = s * gz + dp / hw, whose sums are s * sum(gz) + dp and s * sum(gz*y) + dp/hw * sum(y).
+// One thread-block cluster owns a frame, like gn_bwd_cluster_kernel: each CTA stages its pixel slice in shared memory
+// (slices too large to stage are re-read from global memory), the channel sums go threads -> CTA -> cluster ranks in a
+// fixed order, and every CTA evaluates the excitation on the same totals in the same order, so all hold the same s.
+struct SeP {
+  const float *w1, *b1, *w2, *b2;  // excite.0 weight [cr, C], bias [cr]; excite.2 weight [C, cr], bias [C]
+  const float *s_in, *h_in;        // backward: the forward's s [B, C] and h [B, cr]
+  float *p, *h, *s;                // forward: squeeze [B, C], hidden [B, cr], scale [B, C]
+  float *a, *dh;                   // backward: a = ds * s * (1 - s) [B, C], dh [B, cr]
+  int cr;
+};
+
+// mean / rstd of channel c of frame b (the arithmetic of gn_coeffs)
+__device__ __forceinline__ void gn_chan(const GnP& p, int b, int c, float& mu, float& rs) {
+  const double2 st = *reinterpret_cast<const double2*>(p.stats + ((size_t)b * p.G + (c >> p.lcpg)) * 2);
+  const double md = st.x * (double)p.inv_m;
+  mu = (float)md;
+  rs = rsqrtf(fmaxf((float)(st.y * (double)p.inv_m - md * md), 0.f) + p.eps);
+}
+
+// dst[c] = sum of v over the CTA's pixel lanes (thread = (vec = tid % cv, lane = tid / cv)), added in lane order
+__device__ __forceinline__ void se_cta_chan_sum(const float (&v)[8], float (*sred)[9], float* dst, int C) {
+  const int cv = C >> 3, npl = 256 / cv;
+#pragma unroll
+  for (int e = 0; e < 8; ++e) sred[threadIdx.x][e] = v[e];
+  __syncthreads();
+  for (int c = threadIdx.x; c < C; c += 256) {
+    float t = 0.f;
+    for (int q = 0; q < npl; ++q) t += sred[q * cv + (c >> 3)][c & 7];
+    dst[c] = t;
+  }
+  __syncthreads();
+}
+
+// tot[i] = sum over the cluster's CTAs, in rank order, of their part[i] (i < n).  Ends with a cluster barrier ARRIVE;
+// the caller executes the matching WAIT before it exits, so no CTA leaves while a peer still reads its part.
+__device__ __forceinline__ void se_cluster_total(cg::cluster_group& cluster, const float* part, float* tot, int n,
+                                                 int CS) {
+  cluster.sync();
+  for (int i = threadIdx.x; i < n; i += 256) {
+    float t = 0.f;
+    for (int r = 0; r < CS; ++r) t += cluster.map_shared_rank(part, r)[i];
+    tot[i] = t;
+  }
+  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
+  __syncthreads();
+}
+
+__global__ void __launch_bounds__(256)
+gn_se_residual_relu_kernel(const act_t* __restrict__ y, GnP p, const act_t* __restrict__ res, GnP rp,
+                           int res_is_prenorm, SeP se, act_t* __restrict__ out, grad_t* __restrict__ out2, int hw,
+                           int ppc, int staged) {
+  extern __shared__ __align__(16) uint8_t gsm[];
+  __shared__ float sred[256][9];
+  cg::cluster_group cluster = cg::this_cluster();
+  const int CS = (int)cluster.num_blocks(), rank = (int)cluster.block_rank();
+  const int b = blockIdx.x / CS;
+  const int C = p.C, cv = C >> 3, cr = se.cr, tid = threadIdx.x;
+  const int pix0 = rank * ppc, pix1 = min(hw, pix0 + ppc);
+  const int n = max(pix1 - pix0, 0) * cv;
+  const size_t base = ((size_t)b * hw + pix0) * cv;
+  const uint4* gy = reinterpret_cast<const uint4*>(y) + base;
+  uint4* sy = reinterpret_cast<uint4*>(gsm);
+  float* part = reinterpret_cast<float*>(gsm + (staged ? (size_t)ppc * C * 2 : 0));  // [C] this CTA's sums of y
+  float* tot = part + C;                                                                // [C] the frame's sums
+  float* pv = tot + C;                                                                  // [C] squeeze
+  float* sv = pv + C;                                                                   // [C] scale
+  float* hv = sv + C;                                                                   // [cr] hidden
+  if (staged) {   // every thread later consumes exactly the vectors it copied: no block barrier before use
+    const uint32_t ay = smem_u32(sy);
+    for (int i = tid; i < n; i += 256) cp_async16(ay + i * 16, gy + i, true);
+    cp_async_commit();
+  }
+  const uint4* src = staged ? sy : gy;
+  const int vec = tid % cv, c0 = vec << 3;
+  float zc[8], zd[8], rsc[8], rsh[8];
+  {
+    float mu[8], rs[8], ga[8], be[8];
+    gn_coeffs(p, b, c0, mu, rs);
+    load8f(p.gamma + c0, ga);
+    load8f(p.beta + c0, be);
+#pragma unroll
+    for (int e = 0; e < 8; ++e) { zc[e] = rs[e] * ga[e]; zd[e] = fmaf(-mu[e], zc[e], be[e]); rsc[e] = 1.f; rsh[e] = 0.f; }
+    if (res_is_prenorm) {
+      gn_coeffs(rp, b, c0, mu, rs);
+      load8f(rp.gamma + c0, ga);
+      load8f(rp.beta + c0, be);
+#pragma unroll
+      for (int e = 0; e < 8; ++e) { rsc[e] = rs[e] * ga[e]; rsh[e] = fmaf(-mu[e], rsc[e], be[e]); }
+    }
+  }
+  if (staged) cp_async_wait<0>();
+  float acc[8];
+#pragma unroll
+  for (int e = 0; e < 8; ++e) acc[e] = 0.f;
+  for (int i = tid; i < n; i += 256) {
+    float x[8];
+    unpack8a(src[i], x);
+#pragma unroll
+    for (int e = 0; e < 8; ++e) acc[e] += x[e];
+  }
+  se_cta_chan_sum(acc, sred, part, C);
+  se_cluster_total(cluster, part, tot, C, CS);
+  const float inv_hw = 1.f / (float)hw;
+  for (int c = tid; c < C; c += 256) {
+    float mu, rs;
+    gn_chan(p, b, c, mu, rs);
+    const float k = rs * p.gamma[c];
+    pv[c] = fmaf(tot[c] * inv_hw, k, fmaf(-mu, k, p.beta[c]));
+  }
+  __syncthreads();
+  // excite.0 + ReLU: one warp per hidden unit, lanes stride over C, fixed shuffle tree
+  const int lane = tid & 31, warp = tid >> 5;
+  for (int j = warp; j < cr; j += 8) {
+    const float* w = se.w1 + (size_t)j * C;
+    float t = 0.f;
+    for (int c = lane; c < C; c += 32) t = fmaf(__ldg(w + c), pv[c], t);
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) t += __shfl_xor_sync(0xffffffffu, t, o);
+    if (lane == 0) hv[j] = fmaxf(t + __ldg(se.b1 + j), 0.f);
+  }
+  __syncthreads();
+  // excite.2 + sigmoid: one thread per channel, its weight row in order
+  for (int c = tid; c < C; c += 256) {
+    const float4* w = reinterpret_cast<const float4*>(se.w2 + (size_t)c * cr);
+    float t = __ldg(se.b2 + c);
+    for (int j = 0; j < cr; j += 4) {
+      const float4 wv = __ldg(w + (j >> 2));
+      t = fmaf(wv.x, hv[j], t);
+      t = fmaf(wv.y, hv[j + 1], t);
+      t = fmaf(wv.z, hv[j + 2], t);
+      t = fmaf(wv.w, hv[j + 3], t);
+    }
+    sv[c] = 1.f / (1.f + expf(-t));
+  }
+  __syncthreads();
+  if (rank == 0) {
+    for (int c = tid; c < C; c += 256) {
+      se.p[(size_t)b * C + c] = pv[c];
+      se.s[(size_t)b * C + c] = sv[c];
+    }
+    for (int j = tid; j < cr; j += 256) se.h[(size_t)b * cr + j] = hv[j];
+  }
+  float sc[8];
+#pragma unroll
+  for (int e = 0; e < 8; ++e) sc[e] = sv[c0 + e];
+  const uint4* gr = reinterpret_cast<const uint4*>(res) + base;
+  uint4* go = reinterpret_cast<uint4*>(out) + base;
+  uint4* go2 = out2 ? reinterpret_cast<uint4*>(out2) + base : nullptr;
+  for (int i = tid; i < n; i += 256) {
+    float x[8], r[8];
+    unpack8a(src[i], x);
+    unpack8a(gr[i], r);
+#pragma unroll
+    for (int e = 0; e < 8; ++e) x[e] = fmaxf(fmaf(sc[e], fmaf(x[e], zc[e], zd[e]), fmaf(r[e], rsc[e], rsh[e])), 0.f);
+    go[i] = pack8a(x);
+    if (go2) go2[i] = pack8(x);
+  }
+  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
+}
+
+// Backward of gn_se_residual_relu_kernel's main branch: dy (grad wrt y), gz_out = g * [o > 0] (the residual branch's
+// gradient), the frame's row of the dgamma / dbeta partials [B][C], and the excitation's a [B,C] / dh [B,cr] from which
+// the caller forms the excitation weight gradients.
+__global__ void __launch_bounds__(256)
+gn_se_bwd_kernel(const grad_t* __restrict__ g, const act_t* __restrict__ act, const act_t* __restrict__ y, GnP p,
+                 SeP se, float* __restrict__ dgamma, float* __restrict__ dbeta, grad_t* __restrict__ dy,
+                 grad_t* __restrict__ gz_out, int hw, int ppc, int staged) {
+  extern __shared__ __align__(16) uint8_t gsm[];
+  __shared__ float sred[256][9];
+  cg::cluster_group cluster = cg::this_cluster();
+  const int CS = (int)cluster.num_blocks(), rank = (int)cluster.block_rank();
+  const int b = blockIdx.x / CS;
+  const int C = p.C, G = p.G, cv = C >> 3, cr = se.cr, tid = threadIdx.x;
+  const int pix0 = rank * ppc, pix1 = min(hw, pix0 + ppc);
+  const int n = max(pix1 - pix0, 0) * cv, ncap = staged ? ppc * cv : 0;
+  const size_t base = ((size_t)b * hw + pix0) * cv;
+  const uint4* gg = reinterpret_cast<const uint4*>(g) + base;
+  const uint4* gy = reinterpret_cast<const uint4*>(y) + base;
+  const uint4* ga = reinterpret_cast<const uint4*>(act) + base;
+  uint4* sg = reinterpret_cast<uint4*>(gsm);
+  uint4* sy = sg + ncap;
+  uint4* sa = sy + ncap;
+  float* part = reinterpret_cast<float*>(sa + ncap);  // [3C] this CTA's sum gz, sum gz*y, sum y
+  float* tot = part + 3 * C;                           // [3C] the frame's
+  float* av = tot + 3 * C;                             // [C] a
+  float* dpv = av + C;                                 // [C] dp / hw
+  float* t1 = dpv + C;                                 // [C] sum dz
+  float* t2 = t1 + C;                                  // [C] sum dz * xhat
+  float* red = t2 + C;                                 // [256] partial dot products of dh
+  float* dhv = red + 256;                              // [cr]
+  float* gS = dhv + cr;                                // [2G]
+  if (staged) {
+    const uint32_t ag = smem_u32(sg), ay = smem_u32(sy), aa = smem_u32(sa);
+    for (int i = tid; i < n; i += 256) {
+      cp_async16(ag + i * 16, gg + i, true);
+      cp_async16(ay + i * 16, gy + i, true);
+      cp_async16(aa + i * 16, ga + i, true);
+    }
+    cp_async_commit();
+  }
+  const uint4 *srg = staged ? sg : gg, *sry = staged ? sy : gy, *sra = staged ? sa : ga;
+  const int vec = tid % cv, c0 = vec << 3;
+  if (staged) cp_async_wait<0>();
+  {
+    float s1[8], s2[8], s3[8];
+#pragma unroll
+    for (int e = 0; e < 8; ++e) { s1[e] = 0.f; s2[e] = 0.f; s3[e] = 0.f; }
+    for (int i = tid; i < n; i += 256) {
+      float gv[8], x[8], ac[8];
+      unpack8(srg[i], gv);
+      unpack8a(sry[i], x);
+      unpack8a(sra[i], ac);
+#pragma unroll
+      for (int e = 0; e < 8; ++e) {
+        const float gz = ac[e] > 0.f ? gv[e] : 0.f;
+        s1[e] += gz;
+        s2[e] = fmaf(gz, x[e], s2[e]);
+        s3[e] += x[e];
+      }
+    }
+    se_cta_chan_sum(s1, sred, part, C);
+    se_cta_chan_sum(s2, sred, part + C, C);
+    se_cta_chan_sum(s3, sred, part + 2 * C, C);
+  }
+  se_cluster_total(cluster, part, tot, 3 * C, CS);
+  const float* sf = se.s_in + (size_t)b * C;
+  for (int c = tid; c < C; c += 256) {
+    float mu, rs;
+    gn_chan(p, b, c, mu, rs);
+    const float k = rs * p.gamma[c], kd = fmaf(-mu, k, p.beta[c]);
+    const float ds = fmaf(k, tot[C + c], kd * tot[c]);   // sum_hw gz * z
+    const float s = sf[c];
+    const float a = ds * s * (1.f - s);
+    av[c] = a;
+    if (rank == 0) se.a[(size_t)b * C + c] = a;
+  }
+  __syncthreads();
+  // dh = (W2^T a) * [h > 0]: thread (j, q) walks the q-th contiguous range of channels; ranges are added in order
+  {
+    const int j = tid % cr, q = tid / cr, per = C / (256 / cr);
+    const float* w = se.w2 + j;
+    float t = 0.f;
+    for (int c = q * per; c < (q + 1) * per; ++c) t = fmaf(__ldg(w + (size_t)c * cr), av[c], t);
+    red[tid] = t;
+  }
+  __syncthreads();
+  if (tid < cr) {
+    float t = 0.f;
+    for (int q = 0; q < 256 / cr; ++q) t += red[q * cr + tid];
+    t = se.h_in[(size_t)b * cr + tid] > 0.f ? t : 0.f;
+    dhv[tid] = t;
+    if (rank == 0) se.dh[(size_t)b * cr + tid] = t;
+  }
+  __syncthreads();
+  const float inv_hw = 1.f / (float)hw;
+  for (int c = tid; c < C; c += 256) {
+    float dp = 0.f;
+    for (int j = 0; j < cr; ++j) dp = fmaf(__ldg(se.w1 + (size_t)j * C + c), dhv[j], dp);
+    const float s = sf[c];
+    const float ta = fmaf(s, tot[c], dp);                              // sum dz
+    const float tx = fmaf(s, tot[C + c], dp * inv_hw * tot[2 * C + c]);  // sum dz * y
+    float mu, rs;
+    gn_chan(p, b, c, mu, rs);
+    const float tb = rs * (tx - mu * ta);                              // sum dz * xhat
+    dpv[c] = dp * inv_hw;
+    t1[c] = ta;
+    t2[c] = tb;
+    if (rank == 0) {   // this frame's row of the dgamma / dbeta partials (summed in order by reduce_partials)
+      dbeta[(size_t)b * C + c] = ta;
+      dgamma[(size_t)b * C + c] = tb;
+    }
+  }
+  __syncthreads();
+  const int cpg = 1 << p.lcpg;
+  for (int gi = tid; gi < G; gi += 256) {
+    float s1 = 0.f, s2 = 0.f;
+    for (int c = gi * cpg; c < (gi + 1) * cpg; ++c) {
+      const float gm = p.gamma[c];
+      s1 = fmaf(gm, t1[c], s1);
+      s2 = fmaf(gm, t2[c], s2);
+    }
+    gS[gi] = s1;
+    gS[G + gi] = s2;
+  }
+  __syncthreads();
+  // dy = zc*dz + (x*c3 + c2) as in gn_bwd_cluster_sums, with dz = s*gz + dp/hw
+  float zc[8], c2[8], c3[8], sc[8], dq[8];
+  {
+    float mu[8], rs[8], gm[8];
+    gn_coeffs(p, b, c0, mu, rs);
+    load8f(p.gamma + c0, gm);
+#pragma unroll
+    for (int e = 0; e < 8; ++e) {
+      const int gi = (c0 + e) >> p.lcpg;
+      const float k2 = rs[e] * p.inv_m * gS[gi], k3 = rs[e] * p.inv_m * gS[G + gi];
+      zc[e] = rs[e] * gm[e];
+      c3[e] = -rs[e] * k3;
+      c2[e] = fmaf(mu[e] * rs[e], k3, -k2);
+      sc[e] = sf[c0 + e];
+      dq[e] = dpv[c0 + e];
+    }
+  }
+  uint4* od = reinterpret_cast<uint4*>(dy) + base;
+  uint4* oz = gz_out ? reinterpret_cast<uint4*>(gz_out) + base : nullptr;
+  for (int i = tid; i < n; i += 256) {
+    float gv[8], x[8], ac[8], gz[8], o[8];
+    unpack8(srg[i], gv);
+    unpack8a(sry[i], x);
+    unpack8a(sra[i], ac);
+#pragma unroll
+    for (int e = 0; e < 8; ++e) {
+      gz[e] = ac[e] > 0.f ? gv[e] : 0.f;
+      o[e] = fmaf(zc[e], fmaf(sc[e], gz[e], dq[e]), fmaf(x[e], c3[e], c2[e]));
+    }
+    od[i] = pack8(o);
+    if (oz) oz[i] = pack8(gz);
+  }
+  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
+}
+
+// Cluster size (CTAs per frame) and pixels per CTA for the SE kernels: the smallest cluster whose staged slice of
+// `ntens` 16-bit tensors is <= 48 KB (as in hb200_gn_bwd), up to the portable maximum of 8.  A slice that with the
+// kernel's `extra` bytes of shared memory exceeds 200 KB is not staged (staged = 0: both passes read global memory).
+static int se_launch(const void* kern, int batch, int hw, int C, int ntens, size_t extra, cudaStream_t st,
+                     cudaLaunchConfig_t* cfg, cudaLaunchAttribute* at, int* ppc, int* staged) {
+  int cs = 1;
+  size_t slice = 0;
+  for (;; cs *= 2) {
+    *ppc = (hw + cs - 1) / cs;
+    slice = (size_t)ntens * *ppc * C * 2;
+    if (slice <= 48 * 1024 || cs == 8) break;
+  }
+  *staged = slice + extra <= 200 * 1024 ? 1 : 0;
+  const size_t smem = (*staged ? slice : 0) + extra;
+  HB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  *cfg = {};
+  cfg->gridDim = dim3((unsigned)batch * cs);
+  cfg->blockDim = dim3(256);
+  cfg->dynamicSmemBytes = smem;
+  cfg->stream = st;
+  at[0].id = cudaLaunchAttributeClusterDimension;
+  at[0].val.clusterDim.x = cs; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
+  cfg->attrs = at;
+  cfg->numAttrs = 1;
+  return HB200_OK;
+}
+
+static int se_check(int C, int cr) {
+  HB_CHECK_ARG(C / 8 >= 1 && C / 8 <= 256 && 256 % (C / 8) == 0, "gn_se: C/8 = %d must divide 256", C / 8);
+  HB_CHECK_ARG(cr >= 4 && cr % 4 == 0 && 256 % cr == 0 && C % (256 / cr) == 0,
+               "gn_se: reduced width %d must be a multiple of 4 dividing 256 (and 256/%d must divide C = %d)", cr, cr, C);
+  return HB200_OK;
+}
+
 }  // namespace hb200
 
 using namespace hb200;
@@ -2076,6 +2436,69 @@ extern "C" int hb200_gn_bwd(const hb200_bf16* g, const hb200_bf16* act, const hb
       (const grad_t*)g, (const act_t*)act, (const act_t*)y, p, part_g, part_b,
       (grad_t*)dy, (grad_t*)gz_out, batch, hw, mask_mode);
   HB_LAUNCH_OK();
+  count_launch(1);
+  return gn_affine_grads_reduce(part_g, part_b, batch, channels, dgamma, dbeta, (cudaStream_t)stream);
+}
+
+extern "C" int hb200_gn_se_residual_relu(const hb200_f16* y, const double* stats, const float* gamma,
+                                         const float* beta, const hb200_f16* res, const double* res_stats,
+                                         const float* res_gamma, const float* res_beta, const float* w1,
+                                         const float* b1, const float* w2, const float* b2, float* p, float* h,
+                                         float* s, hb200_f16* out, hb200_bf16* out_bf16, int batch, int hw,
+                                         int channels, int groups, int reduced, float eps, hb200_stream_t stream) {
+  GnP gp, rp;
+  int rc = make_gn(gp, stats, gamma, beta, channels, groups, hw, eps);
+  if (rc) return rc;
+  HB_CHECK_ARG(y && res && out && w1 && b1 && w2 && b2 && p && h && s && batch > 0 && hw > 0,
+               "gn_se_residual_relu: bad args");
+  rc = se_check(channels, reduced);
+  if (rc) return rc;
+  rp = gp;
+  if (res_stats) {
+    rc = make_gn(rp, res_stats, res_gamma, res_beta, channels, groups, hw, eps);
+    if (rc) return rc;
+  }
+  SeP se = {};
+  se.w1 = w1; se.b1 = b1; se.w2 = w2; se.b2 = b2; se.p = p; se.h = h; se.s = s; se.cr = reduced;
+  const size_t extra = sizeof(float) * (4 * (size_t)channels + reduced);
+  cudaLaunchConfig_t cfg;
+  cudaLaunchAttribute at[1];
+  int ppc = 0, staged = 0;
+  auto kern = gn_se_residual_relu_kernel;
+  rc = se_launch((const void*)kern, batch, hw, channels, 1, extra, (cudaStream_t)stream, &cfg, at, &ppc, &staged);
+  if (rc) return rc;
+  HB_CUDA(cudaLaunchKernelEx(&cfg, kern, (const act_t*)y, gp, (const act_t*)res, rp, res_stats ? 1 : 0, se,
+                             (act_t*)out, (grad_t*)out_bf16, hw, ppc, staged));
+  count_launch(1);
+  return HB200_OK;
+}
+
+extern "C" int hb200_gn_se_bwd(const hb200_bf16* g, const hb200_bf16* act, const hb200_bf16* y, const double* stats,
+                               const float* gamma, const float* beta, const float* s, const float* h, const float* w1,
+                               const float* w2, float* dgamma, float* dbeta, hb200_bf16* dy, hb200_bf16* gz_out,
+                               float* a, float* dh, int batch, int hw, int channels, int groups, int reduced,
+                               float eps, hb200_stream_t stream) {
+  GnP gp;
+  int rc = make_gn(gp, stats, gamma, beta, channels, groups, hw, eps);
+  if (rc) return rc;
+  HB_CHECK_ARG(g && act && y && s && h && w1 && w2 && dgamma && dbeta && dy && a && dh && batch > 0 && hw > 0,
+               "gn_se_bwd: bad args");
+  rc = se_check(channels, reduced);
+  if (rc) return rc;
+  float *part_g = nullptr, *part_b = nullptr;
+  rc = gn_affine_grads_workspace((cudaStream_t)stream, batch, channels, &part_g, &part_b);
+  if (rc) return rc;
+  SeP se = {};
+  se.w1 = w1; se.w2 = w2; se.s_in = s; se.h_in = h; se.a = a; se.dh = dh; se.cr = reduced;
+  const size_t extra = sizeof(float) * (10 * (size_t)channels + 256 + reduced + 2 * (size_t)groups);
+  cudaLaunchConfig_t cfg;
+  cudaLaunchAttribute at[1];
+  int ppc = 0, staged = 0;
+  auto kern = gn_se_bwd_kernel;
+  rc = se_launch((const void*)kern, batch, hw, channels, 3, extra, (cudaStream_t)stream, &cfg, at, &ppc, &staged);
+  if (rc) return rc;
+  HB_CUDA(cudaLaunchKernelEx(&cfg, kern, (const grad_t*)g, (const act_t*)act, (const act_t*)y, gp, se, part_g, part_b,
+                             (grad_t*)dy, (grad_t*)gz_out, hw, ppc, staged));
   count_launch(1);
   return gn_affine_grads_reduce(part_g, part_b, batch, channels, dgamma, dbeta, (cudaStream_t)stream);
 }

@@ -266,6 +266,30 @@ def gn_bwd(g, act, y, stats, gamma, beta, dgamma, dbeta, dy, gz_out, batch, hw, 
          ptr(dy), ptr(gz_out), batch, hw, channels, groups, float(eps), mask_mode)
 
 
+def gn_se_residual_relu(y, stats, gamma, beta, res, w1, b1, w2, b2, p, h, s, out, batch, hw, channels, groups,
+                        res_stats=None, res_gamma=None, res_beta=None, eps=1e-5, out_bf16=None):
+    """out = relu(SE(GN(y)) + res); p / h / s f32 [B,C] / [B,C/16] / [B,C] are kept for gn_se_bwd (see hb200.h)"""
+    call("hb200_gn_se_residual_relu", ptr(y), ptr(stats), ptr(gamma), ptr(beta), ptr(res), ptr(res_stats),
+         ptr(res_gamma), ptr(res_beta), ptr(w1), ptr(b1), ptr(w2), ptr(b2), ptr(p), ptr(h), ptr(s), ptr(out),
+         ptr(out_bf16), batch, hw, channels, groups, w1.shape[0], float(eps))
+
+
+def gn_se_bwd(g, act, y, stats, gamma, beta, s, h, w1, w2, dgamma, dbeta, dy, gz_out, a, dh, batch, hw, channels,
+              groups, eps=1e-5):
+    call("hb200_gn_se_bwd", ptr(g), ptr(act), ptr(y), ptr(stats), ptr(gamma), ptr(beta), ptr(s), ptr(h), ptr(w1),
+         ptr(w2), ptr(dgamma), ptr(dbeta), ptr(dy), ptr(gz_out), ptr(a), ptr(dh), batch, hw, channels, groups,
+         w1.shape[0], float(eps))
+
+
+def se_excite_wgrad(a, h, p, dh, dw1, db1, dw2, db2):
+    """excitation weight gradients from gn_se_bwd's a / dh and the forward's p / h: dw2 = a^T h, db2 = sum_B a,
+    dw1 = dh^T p, db1 = sum_B dh (fp32 GEMMs and column sums in a fixed order; written, not accumulated)"""
+    linear_bwd_weight(a, h, dw2)
+    colsum(a, db2)
+    linear_bwd_weight(dh, p, dw1)
+    colsum(dh, db1)
+
+
 # ---- dense / rnn / misc -----------------------------------------------------------------------------------
 DENSE_TF32 = True  # dense layers on wgmma tf32 (the reference's cuDNN-RNN precision); False -> fp32 SIMT
 

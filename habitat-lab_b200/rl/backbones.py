@@ -2,10 +2,9 @@
 (resnet18 / resnet50 / resneXt50 / se_resnet50 / se_resneXt50 / se_resneXt101) with the reference's module names, so
 that `state_dict()` keys and shapes interchange with reference checkpoints.
 
-Only resnet18 has sm_90a kernels behind it today (rl/resnet_policy.py builds its own resnet18 holders and the conv
-engine); the Bottleneck families are the SURVEY 8f-2 "next" row.  These holders exist so that the checkpoint contract
-of configs #3 / #4 is pinned now (tests/test_host_api.py checks them against the layouts recorded from the real
-reference in tests/golden/r50_objectnav.pt and rx50_imagenav.pt); they perform no computation."""
+Every backbone here runs on sm_90a kernels: rl/resnet_policy.py's EncoderEngine reads these holders' parameters and runs
+the convolutions, GroupNorms and (for se_*) the squeeze-excite branch itself.  The holders perform no computation; they
+pin the checkpoint contract (tests/test_host_api.py checks them against the layouts recorded from the real reference)."""
 from __future__ import annotations
 
 from typing import List

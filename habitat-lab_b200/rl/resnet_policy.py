@@ -422,10 +422,10 @@ class EncoderEngine:
         hw = tuple((d - 1) // 2 + 1 for d in self.stem.out_hw)  # MaxPool2d(3, 2, 1)
         self.pool_hw = hw
         self.blocks = []   # (main-branch convs, downsample conv or None)
+        self.se = []       # per block: its SE module's excite Sequential (Linear, ReLU, Linear, Sigmoid), or None
         for li in (1, 2, 3, 4):
             for blk in getattr(bb, f"layer{li}"):
-                if hasattr(blk, "se"):
-                    raise NotImplementedError("squeeze-excite backbones (se_resnet50 / se_resneXt*) have no kernels yet")
+                self.se.append(blk.se.excite if hasattr(blk, "se") else None)
                 seq = blk.convs
                 pairs = [(i, i + 1) for i in range(0, len(seq), 3)]   # (conv, GroupNorm) positions: 0-1, 3-4 (, 6-7)
                 convs, cur = [], hw
@@ -500,6 +500,10 @@ class EncoderEngine:
             for i, c in enumerate(convs[:-1]):
                 ws[f"a{j}_{i}"] = e(B, *c.out_hw, c.co)
             ws[f"o{j}"] = e(B, *convs[-1].out_hw, convs[-1].co)
+            if self.se[j] is not None:   # squeeze p, hidden h, scale s (forward); a, dh (backward): f32 per frame
+                C, cr = convs[-1].co, self.se[j][0].out_features
+                for nm, n in (("p", C), ("h", cr), ("s", C)) + ((("a", C), ("dh", cr)) if train else ()):
+                    ws[f"se{nm}{j}"] = torch.empty(B, n, device=dev)
         ncomp, fh, fw = self.enc.output_shape
         ws["feat"] = torch.empty(B, ncomp * fh * fw, device=dev)
         if train:
@@ -594,6 +598,16 @@ class EncoderEngine:
                     ops.gn_apply(yc, sc, c.gamma, c.beta, ws[f"a{j}_{i}"], B, hw, c.co, c.groups, relu=True,
                                  out_bf16=ws.get(f"a{j}_{i}_b"))
                     cur = ws[f"a{j}_{i}"]
+                elif self.se[j] is not None:   # last conv: relu(SE(GN(y)) + r), r = x or GN_d(conv_d(x))
+                    ex = self.se[j]
+                    rkw = {}
+                    if cd is not None:
+                        yd, sd = conv(cd, x)
+                        rkw = dict(res_stats=sd, res_gamma=cd.gamma, res_beta=cd.beta)
+                    ops.gn_se_residual_relu(yc, sc, c.gamma, c.beta, yd if cd is not None else x, ex[0].weight,
+                                            ex[0].bias, ex[2].weight, ex[2].bias, ws[f"sep{j}"], ws[f"seh{j}"],
+                                            ws[f"ses{j}"], ws[f"o{j}"], B, hw, c.co, c.groups,
+                                            out_bf16=ws.get(f"o{j}_b"), **rkw)
                 elif cd is not None:       # last conv: relu(GN(y) + GN_d(conv_d(x)))
                     yd, sd = conv(cd, x)
                     ops.gn_residual_relu(yc, sc, c.gamma, c.beta, yd, ws[f"o{j}"], B, hw, c.co, c.groups, sd,
@@ -635,6 +649,22 @@ class EncoderEngine:
             dy = view(dy_bufs[slot], c)
             gz = view(ws["gz"], c) if want_gz else None
             ops.gn_bwd(g, act, Y(c), ST(c), c.gamma, c.beta, c.gamma.grad, c.beta.grad, dy, gz, B, hw, c.co, c.groups, mode)
+            return dy, gz
+
+        def se_bwd(j, c, g):
+            """gn_bwd(mode 2, want_gz) of an SE block's last conv, then its excitation weight gradients (side stream)"""
+            hw = c.out_hw[0] * c.out_hw[1]
+            slot = dy_turn[0]
+            dy_turn[0] ^= 1
+            side.wait(dy_busy[slot])
+            dy, gz = view(dy_bufs[slot], c), view(ws["gz"], c)
+            ex = self.se[j]
+            ops.gn_se_bwd(g, ws[f"o{j}"], Y(c), ST(c), c.gamma, c.beta, ws[f"ses{j}"], ws[f"seh{j}"], ex[0].weight,
+                          ex[2].weight, c.gamma.grad, c.beta.grad, dy, gz, ws[f"sea{j}"], ws[f"sedh{j}"], B, hw, c.co,
+                          c.groups)
+            with side.after_main():
+                ops.se_excite_wgrad(ws[f"sea{j}"], ws[f"seh{j}"], ws[f"sep{j}"], ws[f"sedh{j}"], ex[0].weight.grad,
+                                    ex[0].bias.grad, ex[2].weight.grad, ex[2].bias.grad)
             return dy, gz
 
         def wgrad(c, x, dy):
@@ -679,7 +709,10 @@ class EncoderEngine:
             xin = ws[f"o{j - 1}"] if j > 0 else ws["x1"]
             xin_b = ws[f"o{j - 1}_b"] if j > 0 else ws["x1_b"]    # bf16 twin: the weight gradients' x operand
             n = len(convs)
-            dyl, gz = gn_bwd(convs[-1], g, ws[f"o{j}"], 2, True)  # g: grad wrt the block output; gz = g * [o > 0]
+            if self.se[j] is not None:
+                dyl, gz = se_bwd(j, convs[-1], g)
+            else:
+                dyl, gz = gn_bwd(convs[-1], g, ws[f"o{j}"], 2, True)  # g: grad wrt the block output; gz = g * [o > 0]
             wgrad(convs[-1], ws[f"a{j}_{n - 2}_b"], dyl)
             cur ^= 1
             ga = like(g_bufs[cur], ws[f"a{j}_{n - 2}"])

@@ -322,6 +322,28 @@ int hb200_gn_bwd(const hb200_bf16* g, const hb200_bf16* act, const hb200_bf16* y
                  hb200_bf16* gz_out, int batch, int hw, int channels, int groups, float eps, int mask_mode,
                  hb200_stream_t stream);
 
+/* Squeeze-excite block output (SEBottleneck, resnet.py:92-110, 155-180), one launch:
+ *   z = GN(y);  p = mean_hw(z) [B,C];  h = relu(w1 p + b1) [B,reduced];  s = sigmoid(w2 h + b2) [B,C];
+ *   out = relu(s * z + res)
+ * w1 f32 [reduced, C], b1 [reduced], w2 [C, reduced], b2 [C] (nn.Linear layout); p, h, s f32 are written for the
+ * backward.  res takes both forms of hb200_gn_residual_relu.  reduced = C / 16 in the reference; it must be a multiple
+ * of 4 that divides 256. */
+int hb200_gn_se_residual_relu(const hb200_f16* y, const double* stats, const float* gamma, const float* beta,
+                              const hb200_f16* res, const double* res_stats, const float* res_gamma,
+                              const float* res_beta, const float* w1, const float* b1, const float* w2,
+                              const float* b2, float* p, float* h, float* s, hb200_f16* out, hb200_bf16* out_bf16,
+                              int batch, int hw, int channels, int groups, int reduced, float eps,
+                              hb200_stream_t stream);
+/* Backward of hb200_gn_se_residual_relu's main branch: g = grad wrt out, act = out (ReLU mask).  Writes dy (grad wrt y),
+ * gz_out = g * [out > 0] (the residual branch's gradient, may be NULL), adds the GroupNorm affine gradients to
+ * dgamma / dbeta (caller zeroes), and writes a = (sum_hw gz * z) * s * (1 - s) [B,C] and dh = (w2^T a) * [h > 0]
+ * [B,reduced]: the excitation weight gradients are dw2 = a^T h, db2 = sum_B a, dw1 = dh^T p, db1 = sum_B dh. */
+int hb200_gn_se_bwd(const hb200_bf16* g, const hb200_bf16* act, const hb200_bf16* y, const double* stats,
+                    const float* gamma, const float* beta, const float* s, const float* h, const float* w1,
+                    const float* w2, float* dgamma, float* dbeta, hb200_bf16* dy, hb200_bf16* gz_out, float* a,
+                    float* dh, int batch, int hw, int channels, int groups, int reduced, float eps,
+                    hb200_stream_t stream);
+
 /* Stem backward in one pass: MaxPool2d(3,2,1) backward (argmax codes from hb200_gn_relu_maxpool) + ReLU backward +
  * GroupNorm backward (resnet.py:244-252).  dpool bf16 [B,H/2,W/2,C] is the gradient of the pooled activation, y / dy
  * bf16 [B,H,W,C] the stem conv output and its gradient; the full-resolution pooled gradient is never written.

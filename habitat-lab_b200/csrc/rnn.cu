@@ -737,6 +737,8 @@ static int lstm_seq_bwd_impl(const float* dh_out, const float* gates, const floa
   HB_CHECK_ARG(dh_out && gates && cs && c0 && w_hh && masks && dgates && workspace && t_steps > 0 && n > 0,
                "lstm_seq_bwd: bad args");
   HB_CHECK_ARG(hidden % kUnits == 0 && hidden % 32 == 0, "lstm_seq_bwd: hidden must be a multiple of 32");
+  // both kernels read the dgates rows of step t back with 16-byte loads for the dh_{t-1} mat-vec
+  HB_CHECK_ARG(((uintptr_t)dgates & 15) == 0, "lstm_seq_bwd: dgates must be 16-byte aligned");
   cudaStream_t st = (cudaStream_t)stream;
   unsigned* counter = (unsigned*)workspace;
   HB_CUDA(cudaMemsetAsync(counter, 0, sizeof(unsigned), st));
@@ -744,7 +746,7 @@ static int lstm_seq_bwd_impl(const float* dh_out, const float* gates, const floa
   HB_CHECK_ARG(smem <= 200 * 1024, "lstm_seq_bwd: n=%d too large for one CTA's shared memory", n);
   const int grid = hidden / kUnits;
   static const bool use_v1 = getenv("HB200_LSTM_V1") != nullptr;
-  if (hidden == 512 && !use_v1 && ((uintptr_t)dgates & 15) == 0) {
+  if (hidden == 512 && !use_v1) {
     const void* k2 = (const void*)lstm_seq_bwd_v2_kernel<512>;
     const size_t smem2 = smem + sizeof(float) * 256;
     void* args2[] = {(void*)&dh_out, (void*)&gates, (void*)&cs, (void*)&c0, (void*)&c0_stride, (void*)&w_hh,
@@ -757,7 +759,7 @@ static int lstm_seq_bwd_impl(const float* dh_out, const float* gates, const floa
     count_launch(1);
     return HB200_OK;
   }
-  HB_CHECK_ARG(!carry_in && !carry_out, "lstm_seq_bwd: time chunks (carry) need hidden == 512 and 16-byte aligned dgates");
+  HB_CHECK_ARG(!carry_in && !carry_out, "lstm_seq_bwd: time chunks (carry) need hidden == 512");
   const void* kern = (const void*)lstm_seq_bwd_kernel;
   if (smem > 48 * 1024) HB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   int rc = coop_check(kern, kSeqThreads, smem, grid);
@@ -959,6 +961,8 @@ extern "C" int hb200_gru_seq_bwd(const float* dh_out, const float* saved, const 
   HB_CHECK_ARG(dh_out && saved && hs && h0 && w_hh && masks && dgx && dgh && workspace && t_steps > 0 && n > 0,
                "gru_seq_bwd: bad args");
   HB_CHECK_ARG(hidden % 32 == 0 && hidden % kUnits == 0, "gru_seq_bwd: hidden must be a multiple of 32");
+  // the dh_{t-1} mat-vec reads the dgh rows of step t back with 16-byte loads
+  HB_CHECK_ARG(((uintptr_t)dgh & 15) == 0, "gru_seq_bwd: dgh must be 16-byte aligned");
   cudaStream_t st = (cudaStream_t)stream;
   unsigned* counter = (unsigned*)workspace;
   HB_CUDA(cudaMemsetAsync(counter, 0, sizeof(unsigned), st));

@@ -425,7 +425,8 @@ int hb200_lstm_seq_fwd(const float* xproj, const float* w_hh, const float* b_hh,
                        const float* h0, long long h0_stride, const float* c0, long long c0_stride,
                        float* hs, float* cs, float* gates_out, int t_steps, int n, int hidden,
                        void* workspace, hb200_stream_t stream);
-/* dh_out [T,n,H] = gradient wrt the layer output; writes dgates [T,n,4H] (= d xproj). */
+/* dh_out [T,n,H] = gradient wrt the layer output; writes dgates [T,n,4H] (= d xproj), which must be 16-byte aligned
+ * (it is read back with 16-byte loads; a misaligned pointer is an argument error). */
 int hb200_lstm_seq_bwd(const float* dh_out, const float* gates, const float* cs, const float* c0,
                        long long c0_stride, const float* w_hh, const uint8_t* masks, float* dgates,
                        int t_steps, int n, int hidden, void* workspace, hb200_stream_t stream);
@@ -440,7 +441,8 @@ int hb200_lstm_seq_bwd_chunk(const float* dh_out, const float* gates, const floa
                              int carry_out, hb200_stream_t stream);
 /* GRU (gate order r,z,n), same persistent cooperative structure.  xproj [T*n,3H] = x W_ih^T + b_ih;
  * saved [T,n,4H] = (r, z, n, W_hn h + b_hn) for backward (NULL in inference).  Backward writes
- * dgx [T,n,3H] = d xproj (-> dW_ih, db_ih, dx) and dgh [T,n,3H] = d(h-side pre-activations) (-> dW_hh, db_hh). */
+ * dgx [T,n,3H] = d xproj (-> dW_ih, db_ih, dx) and dgh [T,n,3H] = d(h-side pre-activations) (-> dW_hh, db_hh); dgh must
+ * be 16-byte aligned (it is read back with 16-byte loads; a misaligned pointer is an argument error). */
 int hb200_gru_seq_fwd(const float* xproj, const float* w_hh, const float* b_hh, const uint8_t* masks,
                       const float* h0, long long h0_stride, float* hs, float* saved, int t_steps, int n, int hidden,
                       void* workspace, hb200_stream_t stream);

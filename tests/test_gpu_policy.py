@@ -360,8 +360,8 @@ def test_full_size_minibatch_is_additive_over_envs(hb):
 
     (m_full, g_full), = run(1)
     (m_again, g_again), = run(1)
-    rerun = (g_again - g_full).norm().item() / g_full.norm().item()
-    assert rerun < 1e-4, f"run-to-run gradient difference {rerun} (only fp32 atomic ordering may differ)"
+    # no kernel on this path adds floats in a run-dependent order: a rerun gives the same bits
+    assert torch.equal(m_again, m_full) and torch.equal(g_again, g_full)
     (m_a, g_a), (m_b, g_b) = run(2)
     assert torch.isfinite(g_full).all() and g_full.abs().max().item() > 0
     torch.testing.assert_close((m_a + m_b) / 2, m_full, rtol=2e-4, atol=1e-6)
@@ -377,8 +377,7 @@ def test_full_size_minibatch_is_additive_over_envs(hb):
 
 def test_lstm_wavefront_matches_sequential(hb, monkeypatch):
     """The two LSTM layers run as a wavefront over 4 time chunks on two streams (forward and backward); chunking must
-    not change the arithmetic: forward outputs bit-identical to the one-launch-per-layer path, gradients identical
-    up to the fp32 atomic ordering of the split-K weight-gradient kernels."""
+    not change the arithmetic: forward outputs, metrics and gradients bit-identical to the one-launch-per-layer path."""
     from habitat_lab_b200.synthetic import fill_rollout_, pointnav_spaces
 
     T, N = 32, 32   # 256 frames per chunk: the same (multi-row-tile) GEMM path as the unchunked projections
@@ -409,10 +408,9 @@ def test_lstm_wavefront_matches_sequential(hb, monkeypatch):
     assert not pol._rnn_wavefront(True, 512, 2, T)
     m_s, v_s, h_s, g_s = run()
     assert torch.equal(v_w, v_s) and torch.equal(h_w, h_s)
-    torch.testing.assert_close(m_w, m_s, rtol=1e-6, atol=1e-7)
+    assert torch.equal(m_w, m_s)
     assert torch.isfinite(g_w).all() and g_w.abs().max().item() > 0
-    rel = (g_w - g_s).norm().item() / g_s.norm().item()
-    assert rel < 1e-5, rel
+    assert torch.equal(g_w, g_s)
 
 
 def test_graphed_actor_replays_act(hb):

@@ -282,12 +282,27 @@ extern "C" int hb200_adv_normalize(float* advantages, long long n, const double*
 //                    HB/rl/ppo/ppo.py:195-250,260-275)
 // =====================================================================================
 constexpr int kMaxA = 8;
+// min / max / clamp that return NaN when an operand is NaN, as torch.min / torch.max / torch.clamp do (fminf / fmaxf
+// return the other operand).  min.NaN / max.NaN (sm_80+) are min / max otherwise: finite inputs give the same bits.
+__device__ __forceinline__ float min_nan(float a, float b) {
+  float d;
+  asm("min.NaN.f32 %0, %1, %2;" : "=f"(d) : "f"(a), "f"(b));
+  return d;
+}
+__device__ __forceinline__ float max_nan(float a, float b) {
+  float d;
+  asm("max.NaN.f32 %0, %1, %2;" : "=f"(d) : "f"(a), "f"(b));
+  return d;
+}
+__device__ __forceinline__ float clamp_nan(float x, float lo, float hi) { return min_nan(max_nan(x, lo), hi); }
 struct LossPartial {  // one per block
   float vl, al, ent, vsum, rsum, nclip, vmin, vmax, rmin, rmax, pad0, pad1;
 };
 
+// (256, 2): loss_grid launches at most two blocks per SM, so each thread may use up to 128 registers (at the
+// default heuristic ptxas capped some instantiations at 64 and spilled)
 template <int NJ>
-__global__ void __launch_bounds__(256)
+__global__ void __launch_bounds__(256, 2)
 ppo_loss_main_kernel(const float* __restrict__ feat, const float* __restrict__ w_act,
                      const float* __restrict__ b_act, const float* __restrict__ w_val,
                      const float* __restrict__ b_val, const int64_t* __restrict__ actions,
@@ -339,8 +354,8 @@ ppo_loss_main_kernel(const float* __restrict__ feat, const float* __restrict__ w
       if (a < A) se += expf(z[a] - mx);
     const float lse = mx + logf(se);
     const int act = (int)actions[f];
-    // an action outside [0, A) has no log-probability (torch's gather device-asserts): poison the frame with NaN so
-    // the loss and every metric show it instead of silently using log_prob = 0
+    // an action outside [0, A) has no log-probability (torch's gather device-asserts): lp = NaN poisons the frame's
+    // loss, ratio metrics and gradients instead of silently using log_prob = 0
     float logp[kMaxA], prob[kMaxA], ent = 0.f, lp = (act >= 0 && act < A) ? 0.f : __int_as_float(0x7fc00000);
 #pragma unroll
     for (int a = 0; a < kMaxA; ++a) {
@@ -352,18 +367,17 @@ ppo_loss_main_kernel(const float* __restrict__ feat, const float* __restrict__ w
       } else { logp[a] = 0.f; prob[a] = 0.f; }
     }
     const float adv = advs[f], ov = old_v[f], ret = rets[f];
-    const float isw = is_coeffs ? fminf(is_coeffs[f], 1.0f) : 1.0f;
+    const float isw = is_coeffs ? min_nan(is_coeffs[f], 1.0f) : 1.0f;
     const float ratio = expf(lp - old_lp[f]);
     const float s1 = adv * ratio;
-    const float s2 = adv * fminf(fmaxf(ratio, 1.0f - clip), 1.0f + clip);
-    // fminf / fmaxf return the non-NaN operand: re-poison explicitly for an out-of-range action
-    const float a_loss = (act >= 0 && act < A) ? -fminf(s1, s2) : __int_as_float(0x7fc00000);
+    const float s2 = adv * clamp_nan(ratio, 1.0f - clip, 1.0f + clip);
+    const float a_loss = -min_nan(s1, s2);
     float v_used = v;
     bool v_live = true;
     if (use_clip_v) {
       const float delta = v - ov;
       v_live = fabsf(delta) < clip;
-      if (!v_live) v_used = ov + fminf(fmaxf(delta, -clip), clip);
+      if (!v_live) v_used = ov + clamp_nan(delta, -clip, clip);
     }
     const float dv = v_used - ret;
     const float v_loss = 0.5f * dv * dv;
@@ -375,12 +389,13 @@ ppo_loss_main_kernel(const float* __restrict__ feat, const float* __restrict__ w
       p.vl += isw * v_loss; p.al += isw * a_loss; p.ent += isw * ent;
       p.vsum += v; p.rsum += ratio;
       p.nclip += (ratio > 1.0f + clip ? 1.f : 0.f) + (ratio < 1.0f - clip ? 1.f : 0.f);
-      p.vmin = fminf(p.vmin, v); p.vmax = fmaxf(p.vmax, v);
-      p.rmin = fminf(p.rmin, ratio); p.rmax = fmaxf(p.rmax, ratio);
+      p.vmin = min_nan(p.vmin, v); p.vmax = max_nan(p.vmax, v);
+      p.rmin = min_nan(p.rmin, ratio); p.rmax = max_nan(p.rmax, ratio);
     }
     if (compute_grads) {
-      // d total / d lp, d total / d v, d total / d H(entropy)   (each already / B)
-      const float g_lp = (s1 <= s2) ? (-adv * ratio) * isw * invB : 0.f;
+      // d total / d lp, d total / d v, d total / d H(entropy)   (each already / B).  torch.min's backward sends the
+      // gradient to both operands when one is NaN, so a NaN s1 or s2 takes the unclipped (NaN) branch.
+      const float g_lp = !(s1 > s2) ? (-adv * ratio) * isw * invB : 0.f;
       const float g_v = v_live ? c_v * dv * isw * invB : 0.f;
       const float g_h = -c_e * isw * invB;
       float dz[kMaxA + 1];
@@ -414,8 +429,8 @@ ppo_loss_main_kernel(const float* __restrict__ feat, const float* __restrict__ w
     for (int w = 1; w < (int)(blockDim.x >> 5); ++w) {
       const LossPartial q = wpart[w];
       r.vl += q.vl; r.al += q.al; r.ent += q.ent; r.vsum += q.vsum; r.rsum += q.rsum; r.nclip += q.nclip;
-      r.vmin = fminf(r.vmin, q.vmin); r.vmax = fmaxf(r.vmax, q.vmax);
-      r.rmin = fminf(r.rmin, q.rmin); r.rmax = fmaxf(r.rmax, q.rmax);
+      r.vmin = min_nan(r.vmin, q.vmin); r.vmax = max_nan(r.vmax, q.vmax);
+      r.rmin = min_nan(r.rmin, q.rmin); r.rmax = max_nan(r.rmax, q.rmax);
     }
     partials[blockIdx.x] = r;
   }
@@ -423,8 +438,9 @@ ppo_loss_main_kernel(const float* __restrict__ feat, const float* __restrict__ w
 
 // dW[a, col] = sum_b dl[b,a] * feat[b,col];  db[a] = sum_b dl[b,a]
 // One partial row per frame slab (blockIdx.y): parts[y][a * H + col] and parts[y][A1 * H + a], summed in order by
-// reduce_partials (no floating-point atomics: the result is the same every run).
-__global__ void __launch_bounds__(256)
+// reduce_partials (no floating-point atomics: the result is the same every run).  (256, 4): up to 64 registers, where
+// ptxas's default choice of 32 spilled the accumulators.
+__global__ void __launch_bounds__(256, 4)
 ppo_heads_wgrad_kernel(const float* __restrict__ feat, const float* __restrict__ dl, int B, int H,
                        int A1, float* __restrict__ parts) {
   float* prow = parts + (size_t)blockIdx.y * A1 * (H + 1);
@@ -474,8 +490,8 @@ __global__ void ppo_loss_finalize_kernel(const LossPartial* __restrict__ partial
   for (int i = 1; i < nblocks; ++i) {
     const LossPartial q = partials[i];
     r.vl += q.vl; r.al += q.al; r.ent += q.ent; r.vsum += q.vsum; r.rsum += q.rsum; r.nclip += q.nclip;
-    r.vmin = fminf(r.vmin, q.vmin); r.vmax = fmaxf(r.vmax, q.vmax);
-    r.rmin = fminf(r.rmin, q.rmin); r.rmax = fmaxf(r.rmax, q.rmax);
+    r.vmin = min_nan(r.vmin, q.vmin); r.vmax = max_nan(r.vmax, q.vmax);
+    r.rmin = min_nan(r.rmin, q.rmin); r.rmax = max_nan(r.rmax, q.rmax);
   }
   const float invB = 1.0f / (float)B;
   metrics[HB200_M_VALUE_LOSS] = r.vl * invB;
@@ -606,7 +622,8 @@ __global__ void clip_adam_kernel(float* __restrict__ p, const float* __restrict_
   const float total_norm = sqrtf(sqnorm[0]);
   if (blockIdx.x == 0 && threadIdx.x == 0 && grad_norm_out) grad_norm_out[0] = total_norm;
   float coef = gscale;
-  if (max_norm > 0.f) coef *= fminf(max_norm / (total_norm + 1e-6f), 1.0f);
+  // a NaN norm makes every parameter NaN, as clip_grad_norm_ does (its clamp propagates NaN)
+  if (max_norm > 0.f) coef *= min_nan(max_norm / (total_norm + 1e-6f), 1.0f);
   const float step_size = lr / bc1;
   const long long n4 = n >> 2;
   float4* p4 = reinterpret_cast<float4*>(p);

@@ -83,7 +83,12 @@ int hb200_adv_normalize(float* advantages, long long n, const double* stats,
  * Outputs: values, log_probs, entropy f32 [B] (any may be NULL); d_features f32 [B,H];
  * d_w_act [A,H], d_b_act [A], d_w_val [H], d_b_val [1] (OVERWRITTEN, not accumulated);
  * metrics f32 [HB200_LOSS_NMETRICS].  compute_grads=0 -> forward/metrics only.
- * workspace: hb200_ppo_loss_workspace_bytes(B,H,A).  A <= 8, H % 32 == 0, H <= 1024.
+ * workspace: hb200_ppo_loss_workspace_bytes(B,H,A).  1 <= A <= 8, H in {32, 64, 128, 256, 512}; anything else is
+ * refused with an argument error.
+ * NaN: min / max / clamp propagate NaN as torch.min / torch.max / torch.clamp do.  A NaN input reaches exactly the
+ * outputs it reaches in the reference's autograd (a NaN old_value or value takes the value-clipped branch, whose value
+ * gradient is 0); an action outside [0, A) has log-probability NaN, which poisons that frame's loss, ratio metrics,
+ * d_features row and the action-head gradients.
  */
 #define HB200_LOSS_NMETRICS 12
 enum {
@@ -111,7 +116,8 @@ int hb200_ppo_loss(const float* features, const float* w_act, const float* b_act
  * read from hyper[0] (LambdaLR mutates lr every update; keeps the launch graph-capturable).
  * step = 1-based Adam step count for bias correction.  max_grad_norm <= 0 disables clipping.
  * grad_scale multiplies grads first (1/world_size when the all-reduce was a SUM).
- * workspace: hb200_clip_adam_workspace_bytes(n).
+ * workspace: hb200_clip_adam_workspace_bytes(n).  A NaN gradient norm makes every parameter and moment NaN when
+ * max_grad_norm > 0, as clip_grad_norm_'s clamp does.
  */
 size_t hb200_clip_adam_workspace_bytes(long long n);
 int hb200_grad_sqnorm(const float* grads, long long n, float grad_scale, float* sqnorm_out,

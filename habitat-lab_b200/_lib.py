@@ -108,6 +108,7 @@ SIGNATURES = {
     "hb200_index_embed_fwd": ("i", "pppii" + "pip" + "ii" + "p"),
     "hb200_index_embed_bwd": ("i", "pppiii" + "p" + "ii" + "p" + "p"),
     "hb200_prep_generic": ("i", "pppp" + "i" + "p" + "iii" + "pppp" + "p"),
+    "hb200_obs_resample": ("i", "ppp" + "ii" + "p"),
 }
 
 

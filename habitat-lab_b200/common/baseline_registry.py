@@ -44,6 +44,14 @@ class BaselineRegistry:
         return cls._register("storage", to_register, name=name)
 
     @classmethod
+    def register_obs_transformer(cls, to_register=None, *, name=None):
+        return cls._register("obs_transformer", to_register, name=name)
+
+    @classmethod
+    def get_obs_transformer(cls, name):
+        return cls.mapping["obs_transformer"].get(name)
+
+    @classmethod
     def get_trainer(cls, name):
         return cls.mapping["trainer"].get(name)
 

@@ -495,6 +495,57 @@ def prep_generic(sources, frame_rows, H, W, scale_shift=None, out=None, out_bf16
          ptr(out_bf16), ptr(stats_acc))
 
 
+# ---- observation transforms -----------------------------------------------------------------------------
+OBS_AREA, OBS_NEAREST, OBS_COPY = 0, 1, 2
+OBS_MAX_KEYS = 8
+
+
+def obs_resample(keys):
+    """Resample and window NHWC image batches, every key in one launch (ResizeShortestEdge / CenterCropper).
+
+    keys: list of (src [B, H, W, C], dst [B, h, w, C], mode, (Hr, Wr), (y0, x0)).  dst receives rows y0 .. y0+h-1 and
+    columns x0 .. x0+w-1 of src resampled to Hr x Wr: OBS_AREA / OBS_NEAREST as F.interpolate(src.float(), (Hr, Wr),
+    mode).to(src.dtype) computes them on the CPU, bit for bit (u8, f32, i32); OBS_COPY needs (Hr, Wr) = (H, W) and
+    copies the window's bits for any dtype.  Every tensor must be a contiguous CUDA tensor; dst may be a view into a
+    larger buffer (e.g. one time slot of the rollout storage) as long as it is contiguous."""
+    if not 1 <= len(keys) <= OBS_MAX_KEYS:
+        raise _lib.Hb200Error(f"obs_resample: {len(keys)} keys (1..{OBS_MAX_KEYS} per launch)")
+    srcs, dsts, desc, batch = [], [], [], None
+    for i, (src, dst, mode, (hr, wr), (y0, x0)) in enumerate(keys):
+        what = f"obs_resample key {i}"
+        if src.dim() != 4 or dst.dim() != 4:
+            raise _lib.Hb200Error(f"{what}: expected 4-D NHWC tensors, got {tuple(src.shape)} -> {tuple(dst.shape)}")
+        if mode not in (OBS_AREA, OBS_NEAREST, OBS_COPY):
+            raise _lib.Hb200Error(f"{what}: unknown mode {mode}")
+        if mode == OBS_COPY:
+            src, dst = src.view(torch.uint8), dst.view(torch.uint8)  # bits of any dtype, as u8 channels
+        elif src.dtype not in _PREP_DTYPE:
+            raise _lib.Hb200Error(f"{what}: dtype {src.dtype} (uint8, float32 or int32)")
+        _chk(src, src.dtype, f"{what} src")
+        _chk(dst, src.dtype, f"{what} dst")
+        if src.device != dst.device:
+            raise _lib.Hb200Error(f"{what}: src on {src.device}, dst on {dst.device}")
+        B, H, W, C = src.shape
+        _, h, w, c = dst.shape
+        batch = B if batch is None else batch
+        if B != batch or dst.shape[0] != B or c != C:
+            raise _lib.Hb200Error(f"{what}: shapes {tuple(src.shape)} -> {tuple(dst.shape)} (batch {batch})")
+        if mode == OBS_COPY and (hr, wr) != (H, W):
+            raise _lib.Hb200Error(f"{what}: copy keeps the size ({H}, {W}), got ({hr}, {wr})")
+        if not (hr >= 1 and wr >= 1 and 0 <= y0 and 0 <= x0 and y0 + h <= hr and x0 + w <= wr):
+            raise _lib.Hb200Error(f"{what}: window ({y0}, {x0}, {h}, {w}) outside the resampled {hr}x{wr} image")
+        if B == 0 or h == 0 or w == 0:
+            raise _lib.Hb200Error(f"{what}: empty tensor {tuple(dst.shape)}")
+        srcs.append(src.data_ptr())
+        dsts.append(dst.data_ptr())
+        desc += [_PREP_DTYPE[src.dtype], mode, H, W, C, int(hr), int(wr), int(y0), int(x0), h, w]
+    n = len(keys)
+    src_a = (ctypes.c_void_p * n)(*srcs)
+    dst_a = (ctypes.c_void_p * n)(*dsts)
+    desc_a = (ctypes.c_int32 * len(desc))(*desc)
+    call("hb200_obs_resample", ctypes.addressof(src_a), ctypes.addressof(dst_a), ctypes.addressof(desc_a), n, batch)
+
+
 # ---- experimental probes (not on the product path) ------------------------------------------------------
 def tma_halo_probe(x, out, b, oh0, ow0, halo_h, halo_w, pad):
     """x bf16 [B,H,W,C] -> out bf16 [C/8, halo_h, halo_w, 8]: one tile's input halo loaded by TMA (see hb200.h)."""

@@ -20,6 +20,7 @@ import numpy as np
 import torch
 
 from ..common.baseline_registry import baseline_registry
+from ..common.obs_transformers import ObsTransformPlan, apply_obs_transforms_obs_space, get_active_obs_transforms
 from ..common.rollout_storage import RolloutStorage
 from ..common.tensor_dict import TensorDict
 from ..synthetic import pointnav_spaces
@@ -67,16 +68,21 @@ class DDPPOConfig:
     force_distributed: bool = False
 
 
-def make_config(num_environments=4, total_num_steps=-1.0, num_updates=2, height=256, width=256, seed=100, **ppo_kw):
-    """A habitat_baselines-shaped config for the synthetic PointNav DD-PPO run (ddppo_pointnav.yaml values)."""
+def make_config(num_environments=4, total_num_steps=-1.0, num_updates=2, height=256, width=256, seed=100,
+                obs_transforms=None, **ppo_kw):
+    """A habitat_baselines-shaped config for the synthetic PointNav DD-PPO run (ddppo_pointnav.yaml values).
+    obs_transforms: {name: config node with `type` and the transformer's fields} (e.g. the ObjectNav YAMLs'
+    resize_shortest_edge + center_cropper, common/obs_transformers.py); height / width are then the raw sensor size."""
     ppo = PPOConfig(**{**dict(ppo_epoch=2, num_mini_batch=2, num_steps=128, max_grad_norm=0.2), **ppo_kw})
+    agent = SimpleNamespace(name="PointNavResNetPolicy", action_distribution_type="categorical")
+    if obs_transforms is not None:
+        agent.obs_transforms = dict(obs_transforms)
     hb = SimpleNamespace(
         trainer_name="ddppo", updater_name="PPO", distrib_updater_name="DDPPO", rollout_storage_name="RolloutStorage",
         num_environments=num_environments, total_num_steps=total_num_steps, num_updates=num_updates,
         log_interval=10, force_blind_policy=False, num_checkpoints=-1, checkpoint_interval=-1,
         checkpoint_folder="data/checkpoints",
-        rl=SimpleNamespace(ppo=ppo, ddppo=DDPPOConfig(), policy={"main_agent": SimpleNamespace(
-            name="PointNavResNetPolicy", action_distribution_type="categorical")}),
+        rl=SimpleNamespace(ppo=ppo, ddppo=DDPPOConfig(), policy={"main_agent": agent}),
         eval=SimpleNamespace(extra_sim_sensors={}),
     )
     habitat = SimpleNamespace(seed=seed, simulator=SimpleNamespace(agents_order=["main_agent"]),
@@ -218,12 +224,17 @@ class PPOTrainer:
         # (ppo_trainer.py:122-134, 246-259)
         self._env_spec = SimpleNamespace(observation_space=obs_space, action_space=act_space,
                                          orig_action_space=self.envs.orig_action_spaces[0])
+        self._create_obs_transforms()
         self._agent = self._create_agent(None)
         if torch.distributed.is_initialized():
             self._agent.init_distributed(find_unused_params=False)
         self._agent.post_init()
         obs = self.envs.reset()
-        self.rollouts.insert_first_observations(TensorDict.from_tree(obs))
+        if self._obs_plan:
+            rest = self._obs_plan.apply_(obs, self.rollouts.buffers["observations"][0])
+            self.rollouts.buffers["observations"].set(0, TensorDict.from_tree(rest), strict=False)
+        else:
+            self.rollouts.insert_first_observations(TensorDict.from_tree(obs))
         n = self.envs.num_envs
         self.current_episode_reward = torch.zeros(n, 1, device=self.device)
         self.running_episode_stats = dict(count=torch.zeros(n, 1, device=self.device),
@@ -231,6 +242,15 @@ class PPOTrainer:
         self.window_episode_stats = collections.defaultdict(lambda: collections.deque(maxlen=ppo_cfg.reward_window_size))
         self._last_checkpoint_percent = -1.0
         self.t_start = time.time()
+
+    def _create_obs_transforms(self):
+        """ppo_trainer.py:110-113: the policy and the storage are built for the transformed observation space.  The
+        active transforms run fused (ObsTransformPlan): one launch per env step writes the transformed keys straight
+        into the rollout storage's next slot."""
+        raw_space = self._env_spec.observation_space
+        self.obs_transforms = get_active_obs_transforms(self.config)
+        self._env_spec.observation_space = apply_obs_transforms_obs_space(raw_space, self.obs_transforms)
+        self._obs_plan = ObsTransformPlan(self.obs_transforms, raw_space)
 
     def _create_agent(self, resume_state, **kwargs) -> SingleAgentAccessMgr:
         """ppo_trainer.py:122-134"""
@@ -299,6 +319,8 @@ class PPOTrainer:
         self.running_episode_stats["reward"] += torch.where(not_done, torch.zeros_like(rewards), self.current_episode_reward)
         self.running_episode_stats["count"] += (~not_done).float()
         self.current_episode_reward.masked_fill_(~not_done, 0.0)
+        if self._obs_plan:   # transformed keys go straight into slot t + 1; insert copies the rest
+            obs = self._obs_plan.apply_(obs, r.buffers["observations"][r.current_rollout_step_idxs[0] + 1])
         r.insert(next_observations=TensorDict.from_tree(obs), next_recurrent_hidden_states=ad.rnn_hidden_states,
                  actions=ad.actions, action_log_probs=ad.action_log_probs, value_preds=ad.values, rewards=rewards,
                  next_masks=not_done)

@@ -532,6 +532,16 @@ int hb200_prep_generic(const void* const* h_srcs, const int* h_dtypes, const int
                        const float* scale_shift, hb200_f16* out, hb200_bf16* out_bf16, double* stats_acc,
                        hb200_stream_t stream);
 
+/* Observation transforms (HB/common/obs_transformers.py ResizeShortestEdge + CenterCropper, HB/utils/common.py
+ * image_resize_shortest_edge / center_crop) for NHWC batches, every key in ONE launch.  src[i]: [batch, H, W, C],
+ * dst[i]: a contiguous [batch, h, w, C] region (normally one time slot of the rollout storage).  desc: HOST array of
+ * n_keys (<= 8) x 11 ints: dtype (0 u8, 1 f32, 2 i32), mode, H, W, C, Hr, Wr, y0, x0, h, w.  Only the window
+ * (y0, x0, h, w) of the image resampled to Hr x Wr is computed.  Modes, each bit-identical to torch on the CPU running
+ * F.interpolate(img.float(), (Hr, Wr), mode).to(dtype): 0 area (adaptive average pooling), 1 nearest; 2 copy
+ * (Hr = H, Wr = W: the window's bits).  Pointers must be aligned to their element size; src and dst must not overlap. */
+int hb200_obs_resample(const void* const* src, void* const* dst, const int32_t* desc, int n_keys, int batch,
+                       hb200_stream_t stream);
+
 /* Not on the product path yet: mechanism probe (verified on hardware) for the TMA halo load of the halo convolutions
  * (NOTES_NEXT.md): loads the halo_h x halo_w halo of the tile whose first output pixel is (oh0, ow0) of frame b from the
  * NHWC bf16 tensor x [batch, h, w, channels] with channels/8 `cp.async.bulk.tensor.4d` box copies (out-of-bounds rows /

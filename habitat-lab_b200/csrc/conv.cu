@@ -16,6 +16,8 @@
 //   layout 0: no-swizzle "interleaved" core matrices: 16-byte vector (row, k8) at
 //             k8 * rows*16 + row*16               (LBO = rows*16, SBO = 128)
 //   layout 1: 128-byte swizzle: (row>>3)*1024 + (row&7)*128 + ((k8 ^ (row&7)) << 4)
+#include <cuda.h>
+
 #include "common.cuh"
 #include "wgmma.cuh"
 
@@ -289,13 +291,16 @@ __global__ void __launch_bounds__(128) conv_igemm_kernel(const ConvArgs a) {
       }
       int lg = 0;  // log2(min(cpg,32)) - 1
       while ((2 << lg) < cpg && lg < 4) ++lg;
+      // fixed inner trip count: bounded by (8 >> lvl) the loop stays rolled over dynamically indexed arrays (local memory)
 #pragma unroll
       for (int lvl = 0; lvl < 4; ++lvl) {
         if (lvl < lg) {
 #pragma unroll
-          for (int i = 0; i < (8 >> lvl); ++i) {
-            s2[i] = s2[2 * i] + s2[2 * i + 1];
-            q2[i] = q2[2 * i] + q2[2 * i + 1];
+          for (int i = 0; i < 8; ++i) {
+            if (i < (8 >> lvl)) {
+              s2[i] = s2[2 * i] + s2[2 * i + 1];
+              q2[i] = q2[2 * i] + q2[2 * i + 1];
+            }
           }
         }
       }
@@ -361,6 +366,222 @@ __global__ void __launch_bounds__(128) conv_igemm_kernel(const ConvArgs a) {
         }
         dst[v] = u;
       }
+    }
+  }
+}
+
+// ---- persistent, warp-specialised variant (learner-sized stride-1 forward and dgrad, gathered C % 64 == 0) ----------
+// An overload of conv_igemm_kernel (template arguments MODE, SPLIT_N).  The gather kernel above issues its own gathers
+// (address arithmetic and predicates for 8 rows per thread per chunk) between its MMAs, and its 128 x 128 tile reads
+// 32 KB from L2 per 2.1 MFLOP.  Here:
+//   warpgroup 0 (one thread)  producer: per K chunk (one filter tap x 64 channels) one TMA im2col box of the activation
+//                             (forward) or gradient (dgrad) in the 128-byte-swizzle K-major layout (LAYOUT 1, byte for
+//                             byte what the gather writes; padding is the TMA unit's zero fill) and one 16 KB bulk copy
+//                             per 128 columns of the packed weight image, into a kWsStages-deep full / empty mbarrier ring
+//   warpgroups 1, 2           consumers: both work on the same CTA tile and read the same stage, each with a 128 x 128
+//                             fp32 accumulator.  SPLIT_N = false: tile 256 pixels x 128 channels, the consumers split M
+//                             and share B; SPLIT_N = true (OC >= 256): 128 x 256, they split N and share A.  Either way
+//                             a 48 KB stage feeds 4.2 MFLOP (85 FLOP per L2 byte, against 64 for the gather kernel)
+// setmaxnreg moves registers from the producer warpgroup to the consumers.  Tiles are strided statically over a grid
+// sized to the SMs.  Every output row sees the MMA sequence and operand bits of the gather kernel, and the epilogue
+// below restates the gather kernel's: the results are bit-identical.  (One shared epilogue function changed the gather
+// kernel's code generation and made its stride-2 parity-class dgrad 10-20 % slower, so each kernel keeps its own.)
+// The im2col box walks output pixels in (frame, row, column) order, the kernel's row order: the map's bounding box
+// spans the window origins (lower corner = the first origin, element strides = the conv stride), the instruction gives
+// the first row's origin and the tap as the im2col offsets.  Stride-1 dgrad is a forward conv over dy with the flipped
+// filter: origin lower corner -(k-1-pad), tap offsets (k-1-s, k-1-r), i.e. ih = oh + pad - r as in the gather.
+constexpr int kWsThreads = 384;
+constexpr int kWsStages = 4;          // 4 x 48 KB ring + 2 x 17 KB transpose buffers: 226 KB of the SM's 227
+constexpr int kWsProducerRegs = 40;   // 128 x 40 + 256 x 232 = 64512 of the SM's 65536 registers
+constexpr int kWsConsumerRegs = 232;
+
+template <int MODE, bool SPLIT_N>
+__global__ void __launch_bounds__(kWsThreads, 1)
+conv_igemm_kernel(const ConvArgs a, const __grid_constant__ CUtensorMap tmap, int lo_w, int lo_h) {
+  constexpr int BN = kMaxBN;
+  extern __shared__ __align__(16) uint8_t smem_raw[];
+  // epilogue: registers -> (stats | + addend) -> fp16 / bf16 NHWC, as in the gather kernel.  Thread t of the calling
+  // warpgroup owns accumulator row t: output row `m` (pixel of frame `ob`, stored only if `row_ok`), columns
+  // [n0, n0 + BN).  `stage_buf` / `bar`: the warpgroup's transpose buffer and named barrier.  (No bias / ReLU: those
+  // launches stay on the gather kernel.)
+  auto epilogue = [&](const float (&acc_t)[BN], int m, int ob, bool row_ok, int n0, float* stage_buf, int bar) {
+    const int lane = threadIdx.x & 31;
+    const int hw = a.OH * a.OW;
+    int seg = 1;  // lanes of a warp that share a frame (power of two), else 1
+    if ((hw & (hw - 1)) == 0) seg = hw < 32 ? hw : 32;
+#pragma unroll
+    for (int col0 = 0; col0 < BN; col0 += 32) {
+      float acc[32];
+      acc_row32(acc_t, col0, stage_buf, acc, bar);
+
+      if (MODE == 0 && a.stats != nullptr) {
+        const int cpg = a.OC / a.gn_groups;  // channels per group (power of two >= 2)
+        float s2[16], q2[16];
+#pragma unroll
+        for (int i = 0; i < 16; ++i) {
+          s2[i] = acc[2 * i] + acc[2 * i + 1];
+          q2[i] = acc[2 * i] * acc[2 * i] + acc[2 * i + 1] * acc[2 * i + 1];
+        }
+        int lg = 0;  // log2(min(cpg,32)) - 1
+        while ((2 << lg) < cpg && lg < 4) ++lg;
+        // the gather kernel's pairwise tree, same additions in the same order.  The inner loop has a fixed trip count:
+        // bounded by (8 >> lvl) it stays a rolled loop over dynamically indexed arrays, i.e. local memory, which at 226
+        // KB of shared memory per SM has almost no L1 behind it
+#pragma unroll
+        for (int lvl = 0; lvl < 4; ++lvl) {
+          if (lvl < lg) {
+#pragma unroll
+            for (int i = 0; i < 8; ++i) {
+              if (i < (8 >> lvl)) {
+                s2[i] = s2[2 * i] + s2[2 * i + 1];
+                q2[i] = q2[2 * i] + q2[2 * i + 1];
+              }
+            }
+          }
+        }
+        const int ng = 16 >> lg;
+#pragma unroll
+        for (int off = 1; off < 32; off <<= 1) {
+          if (off < seg) {
+#pragma unroll
+            for (int i = 0; i < 16; ++i) {
+              if (i < ng) {
+                s2[i] += __shfl_xor_sync(0xffffffffu, s2[i], off);
+                q2[i] += __shfl_xor_sync(0xffffffffu, q2[i], off);
+              }
+            }
+          }
+        }
+        if (row_ok && (lane & (seg - 1)) == 0) {
+          const int g0 = (n0 + col0) / cpg;
+          double* dst = a.stats + ((size_t)ob * a.gn_groups + g0) * 2;
+#pragma unroll
+          for (int i = 0; i < 16; ++i) {
+            if (i < ng) {
+              atomicAdd(dst + 2 * i, (double)s2[i]);
+              atomicAdd(dst + 2 * i + 1, (double)q2[i]);
+            }
+          }
+        }
+      }
+      if (row_ok) {
+        const size_t o = (size_t)m * a.OC + n0 + col0;
+        if (MODE == 1 && a.addend != nullptr) {
+          const uint4* ad = reinterpret_cast<const uint4*>(a.addend + o);
+#pragma unroll
+          for (int v = 0; v < 4; ++v) {
+            float f[8];
+            unpack8(ad[v], f);
+#pragma unroll
+            for (int e = 0; e < 8; ++e) acc[v * 8 + e] += f[e];
+          }
+        }
+        uint4* dst = reinterpret_cast<uint4*>(a.out + o);
+#pragma unroll
+        for (int v = 0; v < 4; ++v) {
+          uint4 u;
+          if (MODE == 0) {  // forward output y: fp16 (saturating)
+            u.x = pack_f16x2(acc[v * 8 + 0], acc[v * 8 + 1]);
+            u.y = pack_f16x2(acc[v * 8 + 2], acc[v * 8 + 3]);
+            u.z = pack_f16x2(acc[v * 8 + 4], acc[v * 8 + 5]);
+            u.w = pack_f16x2(acc[v * 8 + 6], acc[v * 8 + 7]);
+          } else {          // data gradient: bf16
+            u.x = pack_bf16x2(acc[v * 8 + 0], acc[v * 8 + 1]);
+            u.y = pack_bf16x2(acc[v * 8 + 2], acc[v * 8 + 3]);
+            u.z = pack_bf16x2(acc[v * 8 + 4], acc[v * 8 + 5]);
+            u.w = pack_bf16x2(acc[v * 8 + 6], acc[v * 8 + 7]);
+          }
+          dst[v] = u;
+        }
+      }
+    }
+  };
+  constexpr int MT = SPLIT_N ? 1 : 2, NT = SPLIT_N ? 2 : 1;   // 128-row / 128-column sub-tiles of a CTA tile
+  constexpr uint32_t kSub = kTileM * kChunkK * 2;              // one 128-row K-major chunk: 16 KB
+  constexpr uint32_t kABytes = MT * kSub, kStageBytes = (MT + NT) * kSub;
+  __shared__ __align__(8) uint64_t full_bar[kWsStages], empty_bar[kWsStages];
+  const uint32_t sbase = (smem_u32(smem_raw) + 1023u) & ~1023u;   // swizzle atoms are 1024-byte aligned
+  float* const stage_bufs =
+      reinterpret_cast<float*>(smem_raw + (sbase + kWsStages * kStageBytes - smem_u32(smem_raw)));
+  const int tid = threadIdx.x, wg_id = tid >> 7;
+  if (tid == 0) {
+#pragma unroll
+    for (int i = 0; i < kWsStages; ++i) {
+      mbar_init(&full_bar[i], 1);
+      mbar_init(&empty_bar[i], 2);   // one arrival per consumer warpgroup
+    }
+    mbar_fence_init();
+  }
+  __syncthreads();
+  const int mtiles = (a.M + MT * kTileM - 1) / (MT * kTileM), ntiles = a.OC / (NT * kTileM);
+  const int total = mtiles * ntiles;
+  const int first = blockIdx.x, stride = gridDim.x;
+  const int my_n = first < total ? (total - first + stride - 1) / stride : 0;
+  const int hw = a.OH * a.OW;
+
+  if (wg_id == 0) {
+    setmaxnreg_dec<kWsProducerRegs>();
+    if (tid == 0) {
+      const CUtensorMap* const tmap_p = &tmap;   // param-space address, taken in the kernel body
+      int it = 0;
+      for (int i = 0; i < my_n; ++i) {
+        const int tile = first + i * stride;
+        const int mt = tile / ntiles, nt = tile - mt * ntiles;
+        const int m0 = mt * MT * kTileM;
+        const int ob = m0 / hw, rem = m0 - ob * hw;
+        const int oh = rem / a.OW, ow = rem - oh * a.OW;
+        const int w0 = ow * a.stride + lo_w, h0 = oh * a.stride + lo_h;   // the first row's window origin
+        const __nv_bfloat16* wsrc = a.wimg + (size_t)nt * NT * a.nchunks * (kTileM * kChunkK);
+        for (int c = 0; c < a.nchunks; ++c, ++it) {
+          const int st = it % kWsStages;
+          if (it >= kWsStages) mbar_wait(&empty_bar[st], ((it / kWsStages) - 1) & 1);
+          const int k0 = c * kChunkK;
+          const int tap = k0 >> a.cshift, c0 = k0 & (a.SC - 1);
+          const int r = tap / a.kw, s = tap - r * a.kw;
+          const int offw = MODE == 0 ? s : a.kw - 1 - s, offh = MODE == 0 ? r : a.kh - 1 - r;
+          const uint32_t sa = sbase + (uint32_t)st * kStageBytes;
+          mbar_expect_tx(&full_bar[st], kStageBytes);
+          tma_load_im2col_4d(sa, tmap_p, &full_bar[st], c0, w0, h0, ob, (uint16_t)offw, (uint16_t)offh);
+#pragma unroll
+          for (int j = 0; j < NT; ++j)
+            bulk_load_1d(sa + kABytes + j * kSub, wsrc + ((size_t)j * a.nchunks + c) * (kTileM * kChunkK), kSub,
+                         &full_bar[st]);
+        }
+      }
+    }
+  } else {
+    setmaxnreg_inc<kWsConsumerRegs>();
+    // forward: fp16 activations x fp16 weight image; dgrad: bf16 gradients x bf16 transposed weight image
+    constexpr int kT = MODE == 0 ? kF16 : kBF16;
+    const int wgi = wg_id - 1, t = tid & 127;
+    const uint32_t a_off = SPLIT_N ? 0u : (uint32_t)wgi * kSub;
+    const uint32_t b_off = kABytes + (SPLIT_N ? (uint32_t)wgi * kSub : 0u);
+    float* const stage_buf = stage_bufs + wgi * kStageFloats;
+    float acc_t[kMaxBN];
+    int it = 0;
+    for (int i = 0; i < my_n; ++i) {
+      const int tile = first + i * stride;
+      const int mt = tile / ntiles, nt = tile - mt * ntiles;
+      for (int c = 0; c < a.nchunks; ++c, ++it) {
+        const int st = it % kWsStages;
+        mbar_wait(&full_bar[st], (it / kWsStages) & 1);
+        const uint32_t sa = sbase + (uint32_t)st * kStageBytes;
+        wgmma_fence();
+#pragma unroll
+        for (int kk = 0; kk < kChunkK / 16; ++kk)
+          mma128<kMaxBN, kT>(acc_t, kmajor_desc<1>(sa + a_off, kk, kTileM), kmajor_hi<1>(),
+                             kmajor_desc<1>(sa + b_off, kk, kMaxBN), (c > 0 || kk > 0) ? 1u : 0u);
+        wgmma_commit();
+        wgmma_wait<1>();   // the MMAs of chunk c-1 have read their stage: release it to the producer
+        if (c > 0 && t == 0) mbar_arrive(&empty_bar[(it - 1) % kWsStages]);
+      }
+      wgmma_wait<0>();
+      acc_fence(acc_t);
+      if (t == 0) mbar_arrive(&empty_bar[(it - 1) % kWsStages]);
+      const int m = mt * MT * kTileM + (SPLIT_N ? 0 : wgi * kTileM) + t;
+      const bool row_ok = m < a.M;
+      const int n0 = (nt * NT + (SPLIT_N ? wgi : 0)) * kTileM;
+      epilogue(acc_t, m, (row_ok ? m : 0) / hw, row_ok, n0, stage_buf, 1 + wgi);
     }
   }
 }
@@ -653,9 +874,90 @@ static int ilog2(int v) {
 static bool is_pow2(int v) { return v > 0 && (v & (v - 1)) == 0; }
 static int pick_bn(int n) { return n >= kMaxBN ? kMaxBN : n; }
 
+typedef CUresult (*EncodeIm2colFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
+                                   const cuuint64_t*, const int*, const int*, cuuint32_t, cuuint32_t, const cuuint32_t*,
+                                   CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion,
+                                   CUtensorMapFloatOOBfill);
+static EncodeIm2colFn im2col_encode_fn() {
+  static EncodeIm2colFn fn = nullptr;
+  if (fn) return fn;
+  void* p = nullptr;
+  cudaDriverEntryPointQueryResult q;
+  if (cudaGetDriverEntryPoint("cuTensorMapEncodeIm2col", &p, cudaEnableDefault, &q) != cudaSuccess ||
+      q != cudaDriverEntryPointSuccess)
+    return nullptr;
+  fn = (EncodeIm2colFn)p;
+  return fn;
+}
+
+// window origins of the im2col traversal along one spatial dim: first = lower corner, then `step` apart, `n` of them.
+// Forward: origin = o * stride - pad.  Stride-1 dgrad (forward conv over dy, flipped filter): origin = o - (k - 1 - pad)
+static void im2col_corners(int src_dim, int n, int step, int lo, int* lower, int* upper) {
+  *lower = lo;
+  *upper = lo + (n - 1) * step - (src_dim - 1);   // the last origin, relative to the tensor's last element
+}
+
+template <int MODE, bool SPLIT_N>
+static int launch_igemm_ws(const ConvArgs& a, cudaStream_t st) {
+  constexpr int MT = SPLIT_N ? 1 : 2;
+  EncodeIm2colFn enc = im2col_encode_fn();
+  if (!enc) {
+    set_last_error("conv (im2col TMA): cuTensorMapEncodeIm2col is not available from this driver");
+    return HB200_ERR_UNSUPPORTED;
+  }
+  const int step = MODE == 0 ? a.stride : 1;
+  const int lo_h = MODE == 0 ? -a.pad : -(a.kh - 1 - a.pad), lo_w = MODE == 0 ? -a.pad : -(a.kw - 1 - a.pad);
+  int lower[2], upper[2];   // {W, H}
+  im2col_corners(a.SW, a.OW, step, lo_w, &lower[0], &upper[0]);
+  im2col_corners(a.SH, a.OH, step, lo_h, &lower[1], &upper[1]);
+  CUtensorMap tmap;
+  const cuuint64_t dims[4] = {(cuuint64_t)a.SC, (cuuint64_t)a.SW, (cuuint64_t)a.SH, (cuuint64_t)a.B};
+  const cuuint64_t strides[3] = {(cuuint64_t)a.SC * 2, (cuuint64_t)a.SW * a.SC * 2, (cuuint64_t)a.SH * a.SW * a.SC * 2};
+  const cuuint32_t estr[4] = {1u, (cuuint32_t)step, (cuuint32_t)step, 1u};
+  const CUresult r = enc(&tmap, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, (void*)a.src, dims, strides, lower, upper,
+                         (cuuint32_t)kChunkK, (cuuint32_t)(MT * kTileM), estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                         CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) {
+    set_last_error("conv (im2col TMA): cuTensorMapEncodeIm2col failed (%d)", (int)r);
+    return HB200_ERR_CUDA;
+  }
+  // operand ring | one transpose buffer per consumer warpgroup (+ 1024 for the alignment of the base)
+  const size_t smem = (size_t)kWsStages * 3 * kTileM * kChunkK * 2 + 2 * kStageFloats * sizeof(float) + 1024;
+  auto kern = conv_igemm_kernel<MODE, SPLIT_N>;
+  static int grid_cache = 0;
+  if (grid_cache == 0) {
+    HB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    // resident CTAs per SM from the static limits (registers of 384 threads, shared memory)
+    cudaFuncAttributes fa;
+    HB_CUDA(cudaFuncGetAttributes(&fa, (const void*)kern));
+    const int regs = fa.numRegs > 0 ? fa.numRegs : 168;
+    int per_sm = 65536 / (((regs + 7) / 8 * 8) * kWsThreads);
+    const int by_smem = (int)((227 * 1024) / (smem + fa.sharedSizeBytes));
+    if (by_smem < per_sm) per_sm = by_smem;
+    if (per_sm < 1) per_sm = 1;
+    grid_cache = kNumSMs * per_sm;
+  }
+  const int tiles = cdiv(a.M, MT * kTileM) * (a.OC / ((SPLIT_N ? 2 : 1) * kTileM));
+  const int grid = grid_cache < tiles ? grid_cache : tiles;
+  kern<<<grid, kWsThreads, smem, st>>>(a, tmap, lo_w, lo_h);
+  HB_LAUNCH_OK();
+  count_launch(1);
+  return HB200_OK;
+}
+
 template <int MODE>
 static int launch_igemm(ConvArgs a, int BN, cudaStream_t st) {
   a.wbn = BN;
+  // learner-sized stride-1 launches whose gathered tensor comes in whole 64-channel chunks: the persistent im2col TMA
+  // variant.  "Learner-sized" = enough 128 x 128 tiles that the gather kernel would run them full width at two CTAs per
+  // SM.  The gather kernel keeps the actor's few-tile launches, narrow gathers and stride 2: the dgrad has its parity
+  // classes, and the stride-2 forwards (layer3 / layer4 entries) measured no faster on the im2col variant (it supports
+  // them: element strides = the stride)
+  if (g_umma_layout == 1 && BN == kMaxBN && a.SC % kChunkK == 0 && !a.s2_classes && a.stride == 1 &&
+      a.bias == nullptr && !a.relu && 2LL * cdiv(a.M, kTileM) * (a.OC / kMaxBN) > kNumSMs) {
+    if (a.OC >= 2 * kMaxBN) return launch_igemm_ws<MODE, true>(a, st);
+    return launch_igemm_ws<MODE, false>(a, st);
+  }
   // few output rows (the actor's 64-frame batches: 8 row tiles for the 4x4 layers): a 128-wide N tile leaves 16 CTAs on
   // 132 SMs, each walking the whole K serially.  Narrower N tiles (slices of the packed tile, 128B-swizzle layout
   // only) multiply the CTA count; the activation rows are re-gathered per slice out of L2.

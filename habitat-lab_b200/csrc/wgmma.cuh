@@ -241,6 +241,16 @@ __device__ __forceinline__ void fence_proxy_async_smem() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
 
+// registers per thread of the calling warpgroup (warp-specialised kernels: the producer gives, the consumers take)
+template <int R>
+__device__ __forceinline__ void setmaxnreg_dec() {
+  asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R));
+}
+template <int R>
+__device__ __forceinline__ void setmaxnreg_inc() {
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R));
+}
+
 // ---- mbarrier ------------------------------------------------------------------------------------
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
   asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
@@ -294,6 +304,17 @@ __device__ __forceinline__ void tma_load_5d(uint32_t smem_dst, const void* tmap,
       "cp.async.bulk.tensor.5d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6, %7}], [%2];"
       ::"r"(smem_dst), "l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3),
         "r"(c4)
+      : "memory");
+}
+// 4-D im2col load (NHWC tensor, c = channel, w / h = the first pixel's window origin, n = frame): the map's
+// pixelsPerColumn pixels of the bounding-box traversal starting there, each read at (w + off_w, h + off_h)
+__device__ __forceinline__ void tma_load_im2col_4d(uint32_t smem_dst, const void* tmap, uint64_t* bar, int c, int w,
+                                                   int h, int n, uint16_t off_w, uint16_t off_h) {
+  asm volatile(
+      "cp.async.bulk.tensor.4d.shared::cluster.global.im2col.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], "
+      "[%2], {%7, %8};"
+      ::"r"(smem_dst), "l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(bar)), "r"(c), "r"(w), "r"(h), "r"(n),
+        "h"(off_w), "h"(off_h)
       : "memory");
 }
 // 1-D bulk copy global -> shared (16-byte aligned, size a multiple of 16), completion on an mbarrier's transaction count

@@ -158,15 +158,18 @@ int hb200_prep_apply(const uint8_t* rgb, const float* depth, const int32_t* fram
                      const float* scale_shift, hb200_f16* out, hb200_bf16* out_bf16, int s2d,
                      hb200_stream_t stream);
 
-/* SimpleCNN input (HB/rl/models/simple_cnn.py:139-157): rgb/255 and raw depth concatenated, bf16 NHWC
- * [B,H,W,8] (zero padded channels), no pooling; rows gathered through frame_rows */
+/* SimpleCNN input (HB/rl/models/simple_cnn.py:139-157): rgb/255 and raw depth concatenated, fp16 NHWC
+ * [B,H,W,8] (forward values, act_t; channels past c_rgb + c_depth are zero), no pooling; rows gathered through
+ * frame_rows.  The fp16 pack saturates: |depth| > 65504 and +-inf become +-65504, NaN stays NaN.  `out` holds fp16
+ * bits despite its pointer type */
 int hb200_prep_plain(const uint8_t* rgb, const float* depth, const int32_t* frame_rows, int batch, int height,
                      int width, int c_rgb, int c_depth, hb200_bf16* out, hb200_stream_t stream);
 /* backward of conv+bias -> ReLU: dy = g * (out > 0) (out = post-ReLU activation; NULL -> no mask),
  * dbias[C] += per-channel sums of dy (caller zeroes); dy may be NULL (bias gradient only) */
 int hb200_relu_bias_bwd(const hb200_bf16* g, const hb200_bf16* out, hb200_bf16* dy, float* dbias, long long npix,
                         int channels, hb200_stream_t stream);
-/* bf16 NHWC [B,hw,C] -> f32 [B, C*hw] in (c,h,w) order (nn.Flatten of the NCHW map) */
+/* fp16 NHWC [B,hw,C] (a forward activation, act_t; `x` holds fp16 bits despite its pointer type) -> f32 [B, C*hw]
+ * in (c,h,w) order (nn.Flatten of the NCHW map) */
 int hb200_bf16_hwc_to_f32_chw(const hb200_bf16* x, float* out, int batch, int hw, int channels,
                               hb200_stream_t stream);
 
@@ -391,8 +394,7 @@ int hb200_transpose_f32(const float* src, long long ld_src, float* dst, long lon
 /* out_bf16[i] = bf16(x_f16[i]) (n % 8 == 0): the bf16 twin of a forward activation produced by a conv epilogue
  * (SimpleCNN, HB/rl/models/simple_cnn.py:68-93), read by the weight-gradient kernels */
 int hb200_f16_to_bf16(const hb200_f16* x, hb200_bf16* out, long long n, hb200_stream_t stream);
-/* bf16 activations [M,K] (optionally GN+ReLU applied on load: stats/gamma/beta non-NULL with
- * per-row frame = m, K laid out NHWC (hw, C)) -> f32 [M,K].  Feeds visual_fc. */
+/* out[i] = f32(x_bf16[i]) and out_bf16[i] = bf16(x_f32[i]) (round to nearest even), n a positive multiple of 8 */
 int hb200_bf16_to_f32(const hb200_bf16* x, float* out, long long n, hb200_stream_t stream);
 int hb200_f32_to_bf16(const float* x, hb200_bf16* out, long long n, hb200_stream_t stream);
 

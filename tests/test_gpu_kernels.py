@@ -301,11 +301,20 @@ CONV_CASES = [
     (2, 128, 128, 1, 8, 32, 8, 4, 0),     # SimpleCNN conv 1 (depth only), simple_cnn.py:84-96
     (2, 31, 31, 32, 32, 64, 4, 2, 0),     # SimpleCNN conv 2 (odd input, last row/col unused)
     (2, 14, 14, 64, 64, 32, 3, 1, 0),     # SimpleCNN conv 3 (no padding)
+    # SimpleCNN at the reference's RGB-D 256x256 sensors: conv 1 on 4 real channels padded to 8 (forward and weight
+    # gradient; the policy never asks for its data gradient), conv 2 on the 63x63 map, conv 3 on the 30x30 map
+    (2, 256, 256, 4, 8, 32, 8, 4, 0),
+    (2, 63, 63, 32, 32, 64, 4, 2, 0),
+    (2, 30, 30, 64, 64, 32, 3, 1, 0),
+    # SimpleCNN conv 2 on an even input (84x116 frames, H = 4 mod 8): its data gradient takes the parity-class path
+    # (4x4 taps, pad 0, Co = 64); the 256-frame version is below
+    (6, 20, 28, 32, 32, 64, 4, 2, 0),
     # the cases above have < 132 row tiles: the gather kernel slices the packed N tile (32-wide CTAs, the actor's
     # launch shape); these two keep the full-width tiles of the learner's 4096-frame minibatches covered
     (1200, 4, 4, 256, 256, 256, 3, 1, 1),
     (300, 8, 8, 64, 64, 128, 3, 2, 1),
     (64, 4, 4, 256, 256, 256, 3, 1, 1),   # the actor's layer4 launch: 8 row tiles x 8 slices of 32 channels
+    (256, 20, 28, 32, 32, 64, 4, 2, 0),   # SimpleCNN conv 2, even input, 256-frame minibatch: parity-class dgrad
 ]
 
 
@@ -800,7 +809,10 @@ def tgemm_feed(hb, request):
 
 @pytest.mark.parametrize("M,N,K", [(4096, 512, 2048), (4096, 2048, 576), (128, 64, 64), (260, 36, 100),
                                    # one row tile (the actor's batches): deterministic split-K through the workspace
-                                   (64, 512, 2048), (64, 2048, 576), (64, 2048, 512), (3, 36, 260), (128, 512, 4096)])
+                                   (64, 512, 2048), (64, 2048, 576), (64, 2048, 512), (3, 36, 260), (128, 512, 4096),
+                                   # SimpleCNN's Linear(flatten, 512): RGB-D 256x256 (K = 25088) at the actor's 6 frames
+                                   # and a 256-frame minibatch, RGB 84x116 (K = 2464) at 128 frames
+                                   (6, 512, 25088), (256, 512, 25088), (128, 512, 2464)])
 def test_tgemm_tf32(hb, tgemm_feed, M, N, K):
     """wgmma tf32 dense layers: forward (K-major x K-major), data gradient (K-major x N-major) and
     split-K weight gradient (M-major x N-major) vs fp64; tolerance = TF32 operand rounding (2^-11 relative)."""

@@ -98,6 +98,7 @@ SIGNATURES = {
     "hb200_rnn_shift_mask": ("i", "pplpp" + "iii" + "p"),
     "hb200_colsum": ("i", "plplii" + "p"),
     "hb200_relu_bwd": ("i", "pplll" + "i" + "p"),
+    "hb200_gather_rows": ("i", "pppil" + "p"),
     "hb200_f32_chw_to_bf16_hwc": ("i", "pp" + "iii" + "p"),
     "hb200_heads_fwd": ("i", "ppppp" + "iii" + "pp" + "p"),
     "hb200_heads_act": ("i", "pppppp" + "iii" + "pppp" + "p"),

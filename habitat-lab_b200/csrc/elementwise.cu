@@ -2612,3 +2612,31 @@ extern "C" int hb200_bf16_hwc_to_f32_chw(const hb200_bf16* x, float* out, int ba
   count_launch(1);
   return HB200_OK;
 }
+
+// ======================================================================================
+// frozen-encoder learner: the minibatch's cached visual features (rollout rows frame_rows[f]) as one dense [B, F] matrix
+// for the visual_fc GEMM (HB/rl/ddppo/policy/resnet_policy.py:631-645 reads observations["visual_features"])
+// ======================================================================================
+namespace hb200 {
+__global__ void gather_rows_kernel(const float4* __restrict__ src, const int32_t* __restrict__ frame_rows,
+                                   float4* __restrict__ out, int batch, long long vec_per_row) {
+  const long long total = (long long)batch * vec_per_row;
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    const long long f = i / vec_per_row, j = i - f * vec_per_row;
+    out[i] = __ldg(src + (long long)frame_rows[f] * vec_per_row + j);
+  }
+}
+}  // namespace hb200
+
+extern "C" int hb200_gather_rows(const float* src, const int32_t* frame_rows, float* out, int batch,
+                                 long long row_elems, hb200_stream_t stream) {
+  HB_CHECK_ARG(src && frame_rows && out && batch > 0 && row_elems > 0 && row_elems % 4 == 0 &&
+               ((uintptr_t)src % 16) == 0 && ((uintptr_t)out % 16) == 0,
+               "gather_rows: row_elems must be a positive multiple of 4 and both buffers 16-byte aligned");
+  const long long vec = row_elems / 4;
+  gather_rows_kernel<<<grid_for((long long)batch * vec, 256), 256, 0, (cudaStream_t)stream>>>(
+      (const float4*)src, frame_rows, (float4*)out, batch, vec);
+  HB_LAUNCH_OK();
+  count_launch(1);
+  return HB200_OK;
+}

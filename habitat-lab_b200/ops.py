@@ -426,6 +426,16 @@ def relu_bwd(d, y, cols):
     call("hb200_relu_bwd", ptr(d), ptr(y), d.stride(0), y.stride(0), d.shape[0], cols)
 
 
+def gather_rows(src, frame_rows, out):
+    """out[f] = src[frame_rows[f]] for f32 src [R, F] and out [B, F] (both contiguous), frame_rows int32 [B]"""
+    _chk(src, torch.float32, "gather_rows src")
+    _chk(out, torch.float32, "gather_rows out")
+    _chk(frame_rows, torch.int32, "gather_rows frame_rows")
+    if src.dim() != 2 or out.dim() != 2 or out.shape != (frame_rows.numel(), src.shape[1]):
+        raise _lib.Hb200Error(f"gather_rows: src {tuple(src.shape)}, rows {frame_rows.numel()}, out {tuple(out.shape)}")
+    call("hb200_gather_rows", ptr(src), ptr(frame_rows), ptr(out), out.shape[0], out.shape[1])
+
+
 def f32_chw_to_bf16_hwc(x, out, batch, hw, channels):
     call("hb200_f32_chw_to_bf16_hwc", ptr(x), ptr(out), batch, hw, channels)
 

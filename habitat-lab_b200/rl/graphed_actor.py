@@ -8,7 +8,10 @@ into a CUDA graph and replayed once per environment step; only the inputs are co
     out = actor(obs, hidden, prev_actions, masks)      # PolicyActionData; tensors are overwritten by the next call
 
 The packed bf16 weight images the graph reads are refreshed (outside the graph, same buffers) whenever the policy's
-weights_key() changes, i.e. after every optimizer step."""
+weights_key() changes, i.e. after every optimizer step.
+
+With a frozen visual encoder (train_encoder=False) the observations must carry the step's cached `visual_features`:
+the captured step then starts at visual_fc, like the trainer's act() calls."""
 from __future__ import annotations
 
 from typing import Dict
@@ -16,6 +19,7 @@ from typing import Dict
 import torch
 
 from .._lib import Hb200Error
+from .resnet_policy import VISUAL_FEATURES_KEY
 
 
 class GraphedActor:
@@ -23,6 +27,13 @@ class GraphedActor:
                  deterministic: bool = False, warmup: int = 2):
         if not rnn_hidden_states.is_cuda:
             raise Hb200Error("GraphedActor: inputs must be CUDA tensors (no CPU fallback)")
+        net = getattr(policy, "net", None)
+        frozen = net is not None and any(not p.requires_grad for p in net.visual_encoder.parameters())
+        if frozen and VISUAL_FEATURES_KEY not in observations:
+            # the captured step would run the encoder every replay although the rollout already holds its output
+            raise Hb200Error(f"GraphedActor: the policy's visual encoder is frozen (train_encoder=False); pass the "
+                             f"rollout step's {VISUAL_FEATURES_KEY!r} with the observations so the captured act() reads "
+                             "them instead of re-running the encoder")
         self.policy = policy
         self.deterministic = deterministic
         self.obs = {k: v.clone() for k, v in observations.items()}

@@ -28,7 +28,7 @@ import os
 
 from .ppo import DDPPO, PPO  # noqa: F401  (registers the updaters)
 from . import policy as _policy  # noqa: F401  (registers PointNavBaselinePolicy)
-from .resnet_policy import PointNavResNetPolicy  # noqa: F401
+from .resnet_policy import VISUAL_FEATURES_KEY, PointNavResNetPolicy  # noqa: F401
 from .single_agent_access_mgr import SingleAgentAccessMgr
 
 
@@ -65,14 +65,20 @@ class DDPPOConfig:
     rnn_type: str = "LSTM"
     num_recurrent_layers: int = 2
     backbone: str = "resnet18"
+    pretrained_weights: str = "data/ddppo-models/gibson-2plus-resnet50.pth"
+    pretrained: bool = False           # load the whole policy from pretrained_weights
+    pretrained_encoder: bool = False   # load only the visual encoder from pretrained_weights
+    train_encoder: bool = True         # False: freeze the visual encoder and cache its output in the rollout
+    reset_critic: bool = True          # re-draw the critic head after loading pretrained weights
     force_distributed: bool = False
 
 
 def make_config(num_environments=4, total_num_steps=-1.0, num_updates=2, height=256, width=256, seed=100,
-                obs_transforms=None, **ppo_kw):
+                obs_transforms=None, ddppo=None, **ppo_kw):
     """A habitat_baselines-shaped config for the synthetic PointNav DD-PPO run (ddppo_pointnav.yaml values).
     obs_transforms: {name: config node with `type` and the transformer's fields} (e.g. the ObjectNav YAMLs'
-    resize_shortest_edge + center_cropper, common/obs_transformers.py); height / width are then the raw sensor size."""
+    resize_shortest_edge + center_cropper, common/obs_transformers.py); height / width are then the raw sensor size.
+    ddppo: DDPPOConfig field overrides, e.g. dict(pretrained=True, pretrained_weights=path, train_encoder=False)."""
     ppo = PPOConfig(**{**dict(ppo_epoch=2, num_mini_batch=2, num_steps=128, max_grad_norm=0.2), **ppo_kw})
     agent = SimpleNamespace(name="PointNavResNetPolicy", action_distribution_type="categorical")
     if obs_transforms is not None:
@@ -82,7 +88,7 @@ def make_config(num_environments=4, total_num_steps=-1.0, num_updates=2, height=
         num_environments=num_environments, total_num_steps=total_num_steps, num_updates=num_updates,
         log_interval=10, force_blind_policy=False, num_checkpoints=-1, checkpoint_interval=-1,
         checkpoint_folder="data/checkpoints",
-        rl=SimpleNamespace(ppo=ppo, ddppo=DDPPOConfig(), policy={"main_agent": agent}),
+        rl=SimpleNamespace(ppo=ppo, ddppo=DDPPOConfig(**(ddppo or {})), policy={"main_agent": agent}),
         eval=SimpleNamespace(extra_sim_sensors={}),
     )
     habitat = SimpleNamespace(seed=seed, simulator=SimpleNamespace(agents_order=["main_agent"]),
@@ -179,6 +185,7 @@ class PPOTrainer:
         self.num_steps_done = 0
         self._is_distributed = torch.distributed.is_available() and torch.distributed.is_initialized()
         self._last_fps = 0.0
+        self._is_static_encoder = False
         self.timings = collections.defaultdict(float)
 
     # -- helpers mirroring BaseRLTrainer (common/base_trainer.py:226-267)
@@ -233,8 +240,15 @@ class PPOTrainer:
         if self._obs_plan:
             rest = self._obs_plan.apply_(obs, self.rollouts.buffers["observations"][0])
             self.rollouts.buffers["observations"].set(0, TensorDict.from_tree(rest), strict=False)
+        elif self._agent.is_static_encoder:   # VISUAL_FEATURES_KEY is written below
+            self.rollouts.buffers["observations"].set(0, TensorDict.from_tree(obs), strict=False)
         else:
             self.rollouts.insert_first_observations(TensorDict.from_tree(obs))
+        # frozen encoder: still in training mode here, so this first call updates RunningMeanAndVar -- the only update
+        # it ever gets, since rollouts run in eval mode and the learner never calls the encoder (ppo_trainer.py:261-279)
+        self._is_static_encoder = self._agent.is_static_encoder
+        if self._is_static_encoder:
+            self._encode_visual_features(0)
         n = self.envs.num_envs
         self.current_episode_reward = torch.zeros(n, 1, device=self.device)
         self.running_episode_stats = dict(count=torch.zeros(n, 1, device=self.device),
@@ -242,6 +256,14 @@ class PPOTrainer:
         self.window_episode_stats = collections.defaultdict(lambda: collections.deque(maxlen=ppo_cfg.reward_window_size))
         self._last_checkpoint_percent = -1.0
         self.t_start = time.time()
+
+    def _encode_visual_features(self, slot: int) -> None:
+        """The frozen main encoder on the observations of storage slot `slot` (batch N, after the observation transforms
+        wrote them), its output written straight into that slot's VISUAL_FEATURES_KEY (ppo_trainer.py:467-471)."""
+        obs = self.rollouts.buffers["observations"]
+        t0 = time.perf_counter()
+        self.actor_critic.encode_visual_features(obs[slot], obs[VISUAL_FEATURES_KEY][slot])
+        self.timings["visual_features"] += time.perf_counter() - t0
 
     def _create_obs_transforms(self):
         """ppo_trainer.py:110-113: the policy and the storage are built for the transformed observation space.  The
@@ -324,6 +346,8 @@ class PPOTrainer:
         r.insert(next_observations=TensorDict.from_tree(obs), next_recurrent_hidden_states=ad.rnn_hidden_states,
                  actions=ad.actions, action_log_probs=ad.action_log_probs, value_preds=ad.values, rewards=rewards,
                  next_masks=not_done)
+        if self._is_static_encoder:
+            self._encode_visual_features(r.current_rollout_step_idxs[0] + 1)
         r.advance_rollout()
         return self.envs.num_envs
 

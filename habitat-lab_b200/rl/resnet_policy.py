@@ -35,6 +35,7 @@ BF16 = torch.bfloat16   # gradients (g, dy, gz) and the dgrad weight images
 F16 = torch.float16     # forward values: pooled input, conv outputs, activations, forward weight images
 POINTGOAL_UUID = "pointgoal_with_gps_compass"  # IntegratedPointGoalGPSAndCompassSensor.cls_uuid
 IMAGEGOAL_UUID = "imagegoal"
+VISUAL_FEATURES_KEY = "visual_features"   # PointNavResNetNet.PRETRAINED_VISUAL_FEATURES_KEY: a frozen encoder's output
 
 
 @dataclass
@@ -135,6 +136,7 @@ class PointNavResNetNet(nn.Module):
     """Parameter holder + input layout of the reference Net (resnet_policy.py:394-623): one module per sensor with
     the reference's attribute names (checkpoint keys), and `self.segments`: the column layout of the RNN input in the
     reference's concatenation order (:625-763)."""
+    PRETRAINED_VISUAL_FEATURES_KEY = VISUAL_FEATURES_KEY
 
     def __init__(self, observation_space, action_space, hidden_size, num_recurrent_layers, rnn_type, backbone,
                  resnet_baseplanes, normalize_visual_inputs, fuse_keys=None, discrete_actions=True):
@@ -543,11 +545,11 @@ class EncoderEngine:
             ops.conv_dgrad(dy, c.wt, dx, c.shape(B), addend=addend)
 
     # ---- forward -----------------------------------------------------------------------------
-    def forward(self, x0_writer, B, dev, train, wkey=None):
+    def forward(self, x0_writer, B, dev, train, wkey=None, out=None):
         """x0_writer(x0, x0_bf16) fills the pooled / normalised input.  Returns feat f32 [B, C*h*w] in the
-        reference's (c,h,w) flatten order.  `wkey` identifies the weight values: inference calls (act / get_value
-        during a rollout) with an unchanged key reuse the packed weight images instead of re-packing every tensor per
-        step; training forwards always re-pack."""
+        reference's (c,h,w) flatten order, written into `out` (contiguous f32, B * C*h*w elements) when given.  `wkey`
+        identifies the weight values: inference calls (act / get_value during a rollout) with an unchanged key reuse
+        the packed weight images instead of re-packing every tensor per step; training forwards always re-pack."""
         ws = self._ensure(B, dev, train)
         packed = None
         if train:
@@ -618,9 +620,10 @@ class EncoderEngine:
             x = ws[f"o{j}"]
         yc, sc = conv(self.comp, x)
         fhw = self.comp.out_hw[0] * self.comp.out_hw[1]
-        ops.gn_apply(yc, sc, self.comp.gamma, self.comp.beta, ws["feat"], B, fhw, self.comp.co, self.comp.groups,
+        feat = ws["feat"] if out is None else out
+        ops.gn_apply(yc, sc, self.comp.gamma, self.comp.beta, feat, B, fhw, self.comp.co, self.comp.groups,
                      relu=True, chw_flat=True)
-        return ws["feat"]
+        return feat
 
     # ---- backward ----------------------------------------------------------------------------
     def backward(self, d_feat, B, dev):
@@ -827,30 +830,41 @@ class NativeNetPolicy(nn.Module):
     def flatten_parameters_(self):
         """Re-home every parameter in one flat fp32 buffer (and .grad in a second one) so the
         gradient all-reduce, the norm and Adam are single kernels.  Idempotent; re-run
-        automatically after .to()/load_state_dict replaced the storage."""
+        automatically after .to()/load_state_dict replaced the storage.
+
+        Parameters with requires_grad=False (a frozen visual encoder, train_encoder=False) are placed after all the
+        trainable ones and get no gradient: [0, n) of the parameter buffer and the whole gradient buffer hold exactly the
+        trainable parameters, so the all-reduce, the norm and Adam never touch the frozen ones.  With every parameter
+        trainable the layout is registration order, as before."""
         params = list(self.parameters())
         dev = params[0].device
         if dev.type != "cuda":
             raise Hb200Error("hb200 policy must live on a CUDA device (no CPU fallback)")
-        n = sum(p.numel() for p in params)
+        train = [p for p in params if p.requires_grad]
+        order = train + [p for p in params if not p.requires_grad]
         f = self._flat
-        if f is not None and f["params"].device == dev and all(
-                p.data_ptr() == f["params"].data_ptr() + 4 * o and p.grad is not None and
-                p.grad.data_ptr() == f["grads"].data_ptr() + 4 * o for p, o in zip(params, f["offsets"])):
+        if f is not None and f["params"].device == dev and len(f["plist"]) == len(train) and all(
+                p is q for p, q in zip(order, f["all"])) and all(
+                p.data_ptr() == f["params"].data_ptr() + 4 * o and
+                (p.grad is not None and p.grad.data_ptr() == f["grads"].data_ptr() + 4 * o if p.requires_grad
+                 else p.grad is None) for p, o in zip(order, f["all_offsets"])):
             return f
         # every tensor starts on a 16-byte boundary (TF32 / vector kernels read rows as float4)
-        offs, o = [], 0
-        for p in params:
+        offs, o, n = [], 0, 0
+        for i, p in enumerate(order):
             offs.append(o)
             o += (p.numel() + 3) // 4 * 4
+            if i + 1 == len(train):
+                n = o
         flat_p = torch.zeros(o, device=dev)
-        flat_g = torch.zeros(o, device=dev)
-        for p, off in zip(params, offs):
+        flat_g = torch.zeros(n, device=dev)
+        for i, (p, off) in enumerate(zip(order, offs)):
             k = p.numel()
             flat_p[off:off + k].copy_(p.data.reshape(-1))
             p.data = flat_p[off:off + k].view(p.shape)
-            p.grad = flat_g[off:off + k].view(p.shape)
-        self._flat = dict(params=flat_p, grads=flat_g, offsets=offs, n=o, n_real=n, plist=params)
+            p.grad = flat_g[off:off + k].view(p.shape) if i < len(train) else None
+        self._flat = dict(params=flat_p, grads=flat_g, offsets=offs[: len(train)], n=n,
+                          n_real=sum(p.numel() for p in train), plist=train, all=order, all_offsets=offs)
         self.mark_weights_changed()
         return self._flat
 
@@ -859,8 +873,9 @@ class NativeNetPolicy(nn.Module):
         as soon as the RNN backward is done, long before the conv stack's: the distributed updater reduces
         [tail_offset, n) while the encoder backward still runs (rl/ppo.py DDPPO)."""
         f = self.flatten_parameters_()
-        for (name, _), off in zip(self.named_parameters(), f["offsets"]):
-            if name.startswith("net.state_encoder."):
+        names = {id(p): name for name, p in self.named_parameters()}
+        for p, off in zip(f["plist"], f["offsets"]):
+            if names[id(p)].startswith("net.state_encoder."):
                 return off
         return f["n"]
 
@@ -874,7 +889,7 @@ class NativeNetPolicy(nn.Module):
         f = self._flat
         if f is None:
             return None
-        return (self._wver, f["params"].data_ptr(), f["params"]._version, sum(p._version for p in f["plist"]))
+        return (self._wver, f["params"].data_ptr(), f["params"]._version, sum(p._version for p in f["all"]))
 
     def load_state_dict(self, state_dict, strict: bool = True, **kw):
         out = super().load_state_dict(state_dict, strict=strict, **kw)
@@ -1297,11 +1312,41 @@ class PointNavResNetPolicy(NativeNetPolicy):
 
         return write
 
+    def _stored_features(self, obs, rows, B, dev):
+        """The main encoder's output cached in the observations (VISUAL_FEATURES_KEY, a frozen encoder's rollout) as
+        f32 [B, C*h*w]: the step's own rows as they are, a minibatch's rows gathered into one scratch matrix (the
+        visual_fc GEMM reads dense rows)."""
+        vf = obs[VISUAL_FEATURES_KEY]
+        vf = vf.reshape(vf.shape[0], -1)
+        if not isinstance(obs, RolloutObservations) and vf.is_contiguous():
+            return vf
+        feat = self._tmp("visual_features_rows", (B, vf.shape[1]), dev)
+        ops.gather_rows(vf, rows, feat)
+        return feat
+
+    @torch.no_grad()
+    def encode_visual_features(self, observations, out):
+        """Run the main visual encoder alone on a batch of observations ([N, ...] tensors) and write its output into
+        `out` (f32, N x C x h x w, contiguous): what the trainer stores under VISUAL_FEATURES_KEY after every
+        environment step when the encoder is frozen (ppo_trainer.py:261-279, 467-471).  In training mode the
+        RunningMeanAndVar statistics are updated first, as the reference's encoder call does."""
+        obs, rows = _as_rows(observations, out.device)
+        dev = out.device
+        if dev.type != "cuda":
+            raise Hb200Error("hb200 policy: inputs must be CUDA tensors (no CPU fallback)")
+        B = rows.numel()
+        self.flatten_parameters_()
+        write_x0 = self._visual_prep("visual", obs, rows, B, dev, update_stats=self.training)
+        return self._engine_("visual").forward(write_x0, B, dev, False, wkey=self.weights_key(), out=out.view(B, -1))
+
     def _encode(self, name, obs, rows, B, dev, train, rnn_in, col):
         """one encoder + its Linear/ReLU head into columns [col, col + hidden) of the RNN input"""
         enc, fcs = self._encoder(name)
-        write_x0 = self._visual_prep(name, obs, rows, B, dev, update_stats=train and self.training)
-        feat = self._engine_(name).forward(write_x0, B, dev, train, wkey=self.weights_key())
+        if name == "visual" and VISUAL_FEATURES_KEY in obs:
+            feat = self._stored_features(obs, rows, B, dev)
+        else:
+            write_x0 = self._visual_prep(name, obs, rows, B, dev, update_stats=train and self.training)
+            feat = self._engine_(name).forward(write_x0, B, dev, train, wkey=self.weights_key())
         fc = fcs[1]
         ops.linear_fwd(feat, fc.weight, fc.bias, rnn_in[:, col:], relu=True, ldc=rnn_in.stride(0), tf32=True)
         return feat
@@ -1338,7 +1383,7 @@ class PointNavResNetPolicy(NativeNetPolicy):
                     ops.index_embed_fwd(pa, None, mk, net.prev_action_embedding.weight, rnn_in, col, B)
                 elif kind == "imagegoal":
                     feats[sg["key"]] = self._encode(sg["key"], obs, rows, B, dev, train, rnn_in, col)
-        return rnn_in, dict(feats=feats, rnn_in=rnn_in)
+        return rnn_in, dict(feats=feats, rnn_in=rnn_in, stored=VISUAL_FEATURES_KEY in obs)
 
     def _visual_backward(self, d_rnn_in, s, B, dev):
         net = self.net
@@ -1376,6 +1421,8 @@ class PointNavResNetPolicy(NativeNetPolicy):
             with self._side.after_main():
                 ops.linear_bwd_weight(dvis, feat, fc.weight.grad, accumulate=True, tf32=True)
                 ops.colsum(dvis, fc.bias.grad, n_cols=H)
+            if name == "visual" and v["stored"]:   # cached features are inputs: the gradient stops at visual_fc
+                continue
             d_feat = self._tmp(f"d_feat/{name}", tuple(feat.shape), dev)
             ops.linear_bwd_input(dvis, fc.weight, d_feat, tf32=True)
             self._engine_(name).backward(d_feat, B, dev)

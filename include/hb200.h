@@ -467,6 +467,10 @@ int hb200_colsum(const float* x, long long ld, float* out, long long m, int n, i
 /* d[r,c] = 0 where y[r,c] <= 0, c < cols (ReLU backward on a column block; row pitches ld_*) */
 int hb200_relu_bwd(float* d, const float* y, long long ld_d, long long ld_y, long long rows, int cols,
                    hb200_stream_t stream);
+/* out[f, :] = src[frame_rows[f], :] for f < batch (f32 rows of row_elems, a multiple of 4; 16-byte aligned buffers):
+ * the minibatch's cached visual features of a frozen encoder, read from the rollout storage for the visual_fc GEMM */
+int hb200_gather_rows(const float* src, const int32_t* frame_rows, float* out, int batch, long long row_elems,
+                      hb200_stream_t stream);
 /* f32 [B, C*hw] flattened in (c,h,w) order (nn.Flatten of NCHW, resnet_policy.py:587-594)
  * -> bf16 NHWC [B,hw,C]: the gradient of visual_fc's input re-enters the NHWC conv stack */
 int hb200_f32_chw_to_bf16_hwc(const float* x, hb200_bf16* out, int batch, int hw, int channels,

@@ -125,6 +125,19 @@ __device__ __forceinline__ uint4 pack8(const float (&f)[8]) {
 typedef __half act_t;
 typedef __nv_bfloat16 grad_t;
 
+// min / max that return NaN when an operand is NaN, as torch.min / torch.max / torch.relu do (fminf / fmaxf return the
+// other operand).  min.NaN / max.NaN (sm_80+) are min / max otherwise: finite inputs give the same bits.
+__device__ __forceinline__ float min_nan(float a, float b) {
+  float d;
+  asm("min.NaN.f32 %0, %1, %2;" : "=f"(d) : "f"(a), "f"(b));
+  return d;
+}
+__device__ __forceinline__ float max_nan(float a, float b) {
+  float d;
+  asm("max.NaN.f32 %0, %1, %2;" : "=f"(d) : "f"(a), "f"(b));
+  return d;
+}
+
 // fp16 pack with saturation to +-65504 (one F2FP.SATFINITE instruction): an overflow must not become inf
 __device__ __forceinline__ uint32_t pack_f16x2(float lo, float hi) {
   uint32_t r;

@@ -223,7 +223,7 @@ __device__ __forceinline__ void gn_coeffs(const GnP& p, int b, int c0, float (&m
       const double2 st = *reinterpret_cast<const double2*>(p.stats + ((size_t)b * p.G + g) * 2);
       const double md = st.x * (double)p.inv_m;
       m = (float)md;
-      const float var = fmaxf((float)(st.y * (double)p.inv_m - md * md), 0.f);
+      const float var = max_nan((float)(st.y * (double)p.inv_m - md * md), 0.f);   // NaN statistics stay NaN
       r = rsqrtf(var + p.eps);
       prev = g;
     }
@@ -277,7 +277,7 @@ gn_apply_kernel(const act_t* __restrict__ y, GnP p, void* __restrict__ out, grad
 #pragma unroll
     for (int e = 0; e < 8; ++e) {
       const float z = fmaf(x[e], sc[e], sh[e]);
-      x[e] = relu ? fmaxf(z, 0.f) : z;
+      x[e] = relu ? max_nan(z, 0.f) : z;
     }
     if (OUT_F32 == 1) {
       float4* o = reinterpret_cast<float4*>(out) + 2 * i;
@@ -319,7 +319,7 @@ gn_residual_relu_kernel(const act_t* __restrict__ y, GnP p, const act_t* __restr
     unpack8a(reinterpret_cast<const uint4*>(y)[i], x);
     unpack8a(reinterpret_cast<const uint4*>(res)[i], r);
 #pragma unroll
-    for (int e = 0; e < 8; ++e) x[e] = fmaxf(fmaf(x[e], sc[e], sh[e]) + fmaf(r[e], rsc[e], rsh[e]), 0.f);
+    for (int e = 0; e < 8; ++e) x[e] = max_nan(fmaf(x[e], sc[e], sh[e]) + fmaf(r[e], rsc[e], rsh[e]), 0.f);
     reinterpret_cast<uint4*>(out)[i] = pack8a(x);
     if (out2) reinterpret_cast<uint4*>(out2)[i] = pack8(x);
   }
@@ -357,8 +357,8 @@ gn_relu_maxpool_kernel(const act_t* __restrict__ y, GnP p, act_t* __restrict__ o
         unpack8a(*reinterpret_cast<const uint4*>(y + (((size_t)b * H + iy) * W + ix) * p.C + c0), x);
 #pragma unroll
         for (int e = 0; e < 8; ++e) {
-          const float z = fmaxf(fmaf((x[e] - mu[e]) * rs[e], ga[e], be[e]), 0.f);
-          if (z > best[e]) { best[e] = z; arg[e] = r * 3 + s; }
+          const float z = max_nan(fmaf((x[e] - mu[e]) * rs[e], ga[e], be[e]), 0.f);
+          if (z > best[e] || z != z) { best[e] = z; arg[e] = r * 3 + s; }   // MaxPool2d: a NaN tap wins
         }
       }
     }
@@ -402,7 +402,9 @@ gn_relu_maxpool_slab_kernel(const act_t* __restrict__ y, GnP p, act_t* __restric
 #pragma unroll
     for (int e = 0; e < 8; ++e) {
       const float zc = rs[e] * ga[e];
-      sg[e] = zc < 0.f ? -1.f : 1.f;
+      // zc == 0: every tap's value is relu(beta); sg = 0 makes every x * sg equal, so the strict > below keeps the
+      // first valid tap, as MaxPool2d does.  A NaN zc (NaN statistics) makes every tap NaN (sg = zc * 0 = NaN).
+      sg[e] = zc < 0.f ? -1.f : (zc > 0.f ? 1.f : zc * 0.f);
       za[e] = fabsf(zc);
       zd[e] = fmaf(-mu[e], zc, be[e]);
     }
@@ -432,13 +434,13 @@ gn_relu_maxpool_slab_kernel(const act_t* __restrict__ y, GnP p, act_t* __restric
 #pragma unroll
         for (int e = 0; e < 8; ++e) {
           const float xs = x[e] * sg[e];
-          if (xs > best[e]) { best[e] = xs; arg[e] = r * 3 + s; }
+          if (xs > best[e] || xs != xs) { best[e] = xs; arg[e] = r * 3 + s; }   // MaxPool2d: a NaN tap wins
         }
       }
     }
     float z[8];
 #pragma unroll
-    for (int e = 0; e < 8; ++e) z[e] = fmaxf(fmaf(best[e], za[e], zd[e]), 0.f);
+    for (int e = 0; e < 8; ++e) z[e] = max_nan(fmaf(best[e], za[e], zd[e]), 0.f);
     o4[it] = pack8a(z);
     if (o4b) o4b[it] = pack8(z);
     uint2 a;
@@ -643,7 +645,7 @@ __device__ __forceinline__ void gn_bwd_cluster_sums(cg::cluster_group& cluster, 
     const double2 st = *reinterpret_cast<const double2*>(p.stats + ((size_t)b * G + (c >> p.lcpg)) * 2);
     const double md = st.x * (double)p.inv_m;
     const float m = (float)md;
-    const float r = rsqrtf(fmaxf((float)(st.y * (double)p.inv_m - md * md), 0.f) + p.eps);
+    const float r = rsqrtf(max_nan((float)(st.y * (double)p.inv_m - md * md), 0.f) + p.eps);
     const float tb = r * (tx - m * ta);  // sum gz * xhat
     tot[c] = ta;
     tot[C + c] = tb;

@@ -282,18 +282,6 @@ extern "C" int hb200_adv_normalize(float* advantages, long long n, const double*
 //                    HB/rl/ppo/ppo.py:195-250,260-275)
 // =====================================================================================
 constexpr int kMaxA = 8;
-// min / max / clamp that return NaN when an operand is NaN, as torch.min / torch.max / torch.clamp do (fminf / fmaxf
-// return the other operand).  min.NaN / max.NaN (sm_80+) are min / max otherwise: finite inputs give the same bits.
-__device__ __forceinline__ float min_nan(float a, float b) {
-  float d;
-  asm("min.NaN.f32 %0, %1, %2;" : "=f"(d) : "f"(a), "f"(b));
-  return d;
-}
-__device__ __forceinline__ float max_nan(float a, float b) {
-  float d;
-  asm("max.NaN.f32 %0, %1, %2;" : "=f"(d) : "f"(a), "f"(b));
-  return d;
-}
 __device__ __forceinline__ float clamp_nan(float x, float lo, float hi) { return min_nan(max_nan(x, lo), hi); }
 struct LossPartial {  // one per block
   float vl, al, ent, vsum, rsum, nclip, vmin, vmax, rmin, rmax, pad0, pad1;

@@ -292,6 +292,8 @@ int hb200_umma_gemm_probe(const hb200_bf16* a, const hb200_bf16* b, float* d, in
  * replace nn.GroupNorm, nn.ReLU, nn.MaxPool2d and the residual add of BasicBlock
  * (HB/rl/ddppo/policy/resnet.py:37-69, 207-219, 272-281).
  * stats f64 [B,G,2] = (sum, sumsq) over the (C/G)*H*W elements of each group (conv epilogue).
+ * NaN: the ReLU of gn_apply, gn_residual_relu and gn_relu_maxpool propagates NaN as torch.relu does, so a NaN in y
+ * (or res) gives NaN at that element and NaN statistics give NaN over their (frame, group).
  */
 /* out = act(gamma * (y - mu) * rstd + beta);  relu: 0/1;  out_f32: 0 -> bf16 NHWC, 1 -> f32 NHWC,
  * 2 -> f32 [B, C*hw] flattened in (c,h,w) order (what nn.Flatten of the NCHW map feeds visual_fc) */
@@ -305,7 +307,11 @@ int hb200_gn_residual_relu(const hb200_f16* y, const double* stats, const float*
                            const float* res_gamma, const float* res_beta, hb200_f16* out,
                            hb200_bf16* out_bf16, int batch, int hw, int channels, int groups, float eps,
                            hb200_stream_t stream);
-/* out[B,H/2,W/2,C] = maxpool3x3s2p1(relu(GN(y[B,H,W,C]))); argmax u8 (0..8) saved for bwd */
+/* out[B,H/2,W/2,C] = maxpool3x3s2p1(relu(GN(y[B,H,W,C]))); argmax u8 (0..8) saved for bwd.
+ * argmax = r*3+s of the window's first maximum in (r, s) order, as MaxPool2d records it, wherever the pooled value is
+ * > 0 (exact ties included, and a gamma = 0 channel, where every tap equals relu(beta)).  Where every tap is <= 0
+ * after the ReLU the even-H/W kernel may record another tap; the ReLU mask stops the gradient there, so the backward
+ * is the same.  A NaN tap makes the pooled value NaN and the last NaN tap is recorded, as MaxPool2d does. */
 int hb200_gn_relu_maxpool(const hb200_f16* y, const double* stats, const float* gamma,
                           const float* beta, hb200_f16* out, hb200_bf16* out_bf16, uint8_t* argmax, int batch,
                           int h, int w, int channels, int groups, float eps, hb200_stream_t stream);

@@ -517,178 +517,142 @@ conv_halo_wgrad_kernel(const HaloWgradArgs a, const __grid_constant__ CUtensorMa
 
 
 // ------------------------------------------------------------------------------------------
-// weight gradient of the 3x3 pad-1 stride-1 convs on SMALL images (8x8: layer3, 4x4: layer4 / compression).
-// The gather kernel (conv.cu) re-reads x once per tap and dy once per 128-row M tile through L2 (1.2 GB per launch
-// for a 128->128 layer: L2-gather-bound, far below the tensor roofline).  Here the halo scheme of the kernel above
-// is applied to a tile made of SEVERAL images: a 16x8 output tile = 16/IMG images stacked vertically, each with its
-// own zero-padding rows in the halo buffer (and, for 4x4 images, 4 zero "virtual" pixels per 8-pixel row whose dy is
-// zero), so x is loaded once per (channel slice) and every tap is a shifted descriptor.  Channels are sliced to keep
-// the accumulator in registers: a CTA owns 32 input channels (the three vertical taps x 32 channels = 96 rows of
-// one M = 128 tile), NS output channels and ONE horizontal tap s (a 128 x NS accumulator).
-// grid = (tile workers, Ci/32 * Co/NS slices x 3 taps); results are accumulated into dw with vector red.add.
+// weight gradient of the 3x3 pad-1 stride-1 convs on SMALL images (8x8: layer3; 4x4: layer4 / compression; the
+// Bottleneck / ResNeXt 3x3s and the compression of configs #3 / #4).  Per tap (r, s) it is a GEMM with M = input
+// channels (no padding rows), N = output channels and K = output pixels.  A stage is one 16 x 8 output tile, i.e. 16 / IMG
+// stacked images, and a K16 step is two of its 8-column rows, in this order: 16 real pixels (two rows of an 8x8 image),
+// or two 4-pixel rows of a 4x4 image each followed by 4 columns of zero dy.  That is the K grouping, MMA order, tile ->
+// worker assignment and partial layout of the halo tiling earlier versions used, so every fp32 addition is the same and
+// the weight gradients are bit for bit what they were (a 4x4 image per K16 would halve the MMAs at 4x4, but round
+// differently and change the training trajectory).
+//   dy  [64-channel block][pixel][128 B]: TMA box {64 ch, 8 columns, IMG rows, images}, SWIZZLE_128B = the MN-major B
+//       layout; columns 4..7 of a 4x4 image are outside the tensor and zero-filled.
+//   x   [8-channel chunk][image][padded row][pixel][8 ch]: ONE 5-D TMA box of x viewed as (8 ch | column | row | frame |
+//       chunk), columns starting at s - 1 and rows at -1.  The horizontal tap s is thereby pre-shifted into the copy, and
+//       the out-of-bounds fill writes the zero columns of the padding, one zero row above and below every image, the
+//       frames past B (ragged last tile) and the channels past Ci (a 32-channel last block).
+//       A (MN-major, no swizzle) of tap (r, s) starts r rows into an image; its K8 halves start one row apart (LBO =
+//       one row): an 8-pixel row, or a 4-pixel row followed by the next row's 4 pixels, which meet zero dy.  The
+//       8-channel blocks of M sit at the uniform chunk stride (SBO).  The last 4x4 K8 half of a stage reads one row past
+//       its chunk: the next chunk's zero padding row, or after the last chunk a gap zeroed once at the start (TMA never
+//       writes it), so the products there are finite x 0.
+// A CTA owns one (64-channel ci block, horizontal tap s, 128-column co block) slice.  Warp 12 is the producer (one
+// thread issues the TMA into an NS-deep full / empty mbarrier ring); consumer warpgroup r = 0..2 owns tap (r, s) as a
+// 64 x 128 register accumulator that persists over all of the worker's tiles, so one loaded stage feeds three taps.
+// The consumers only issue MMAs and release stages (one wgmma group kept in flight across stage boundaries).  Tiles are
+// strided statically over the workers (blockIdx.x); each worker writes its partial, summed in worker order by
+// reduce_partials: the same result every run.
 // ------------------------------------------------------------------------------------------
-constexpr int kSmallWgradStages = 3;
-struct HaloWgradSmallArgs {
-  const grad_t* x;    // [B, IMG, IMG, Ci]  bf16 twin of the forward activation
-  const grad_t* dy;   // [B, IMG, IMG, Co]  bf16
-  float* dw;          // partials [blockIdx.x][(r*3+s)*Ci + ci][Co], summed in order by reduce_partials
-  int B, Ci, Co, ntiles;
+// 13 warps: three consumer warpgroups and the producer warp.  Accumulators are 64 x 128 (64 registers per thread): a
+// 64 x 256 one spills and serialises the MMAs at the 152 registers 416 threads can have (setmaxnreg needs whole
+// warpgroups, and ptxas allocates within the launch bound anyway).
+constexpr int kWgradSmallThreads = 416;
+constexpr int kWgradSmallCols = 128;   // output channels per CTA slice
+struct WgradSmallArgs {
+  float* dw;   // partials [blockIdx.x][(r*3+s)*Ci + ci][Co], summed in order by reduce_partials
+  int Ci, Co, ntiles;
 };
 
-template <int NS, int IMG>
-__global__ void __launch_bounds__(128)
-conv_halo_wgrad_small_kernel(const HaloWgradSmallArgs a, const __grid_constant__ CUtensorMap tmap_dy) {
-  constexpr int CJ = 4, KH = 3, KW = 3, HWD = TW + KW - 1;
-  constexpr int P = HWD * 16, RP = CJ * P;
-  constexpr int IPT = TH / IMG;                 // images per 16-row tile
-  constexpr int RPI = IMG + 2;                  // halo rows per image (own top / bottom padding row)
-  constexpr int HROWS_LOAD = IPT * RPI;
-  constexpr int HROWS = (IPT - 1) * RPI + (IMG - 2) + 1 + 4;   // last K16 base row + second K8 row + 4 row blocks (M padding)
-  constexpr int HROWS_A = HROWS > HROWS_LOAD ? HROWS : HROWS_LOAD;
-  constexpr int HALO_BYTES = (HROWS_A * RP + 1023) / 1024 * 1024;   // the dy tile behind it must be 1024-byte aligned
-  constexpr int NB = NS / 64;                   // 64-channel (128-byte) column blocks of the dy tile
-  constexpr int DY_BYTES = NB * 128 * 128;      // [block][pixel][128 B], TMA SWIZZLE_128B
-  constexpr int STAGE = HALO_BYTES + DY_BYTES;
-  constexpr int NST = kSmallWgradStages;        // 3-deep ring: the loads of tile it+2 overlap the MMAs of tiles it, it+1
-  static_assert(NS <= 128, "one 128 x NS accumulator per CTA");
-  extern __shared__ __align__(16) uint8_t smem_raw[];
-  __shared__ __align__(8) uint64_t dy_bar[NST];
-  __shared__ float stage_buf[kStageFloats];
-  const uint32_t sbase = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const int tid = threadIdx.x, warp = tid >> 5;
-  const int nsl = a.Co / NS;
-  const int s_tap = blockIdx.y % KW, slice = blockIdx.y / KW;   // horizontal tap of this CTA's accumulator
-  const int c_off = (slice / nsl) * 32, n_off = (slice % nsl) * NS;
-  const CUtensorMap* const tmap_p = &tmap_dy;   // param-space address (see conv_halo_tma_kernel)
+template <int IMG>
+struct WgradSmallCfg {
+  static constexpr int NIMG = TH / IMG;                       // images per stage: one 16 x 8 tile, 8 K16 steps
+  static constexpr int ROWB = IMG * 16;                       // one padded row of one 8-channel chunk
+  static constexpr int CHUNK = NIMG * (IMG + 2) * ROWB;       // one 8-channel chunk of the stage (A's SBO)
+  static constexpr int XB = 8 * CHUNK;                        // 64 input channels
+  static constexpr int DYBLK = TH * TW * 128;                 // one 64-channel block of dy: 128 pixels x 128 B
+  static constexpr int DYB = kWgradSmallCols / 64 * DYBLK;
+  static constexpr int GAP = 1024;                            // zeroed, behind x (the over-read above); keeps alignment
+  static constexpr int STAGE = DYB + XB + GAP;                // dy first: its 1024-byte swizzle atoms stay aligned
+  static constexpr int NS_FIT = (227 * 1024 - 1024 - 256) / STAGE;
+  static constexpr int NS = NS_FIT < 8 ? NS_FIT : 8;
+  static constexpr size_t SMEM = (size_t)NS * STAGE + 1024;
+  static_assert(XB % 1024 == 0 && NS >= 3, "stage layout");
+};
 
+template <int IMG>
+__global__ void __launch_bounds__(kWgradSmallThreads, 1)
+conv_wgrad_small_ws_kernel(const WgradSmallArgs a, const __grid_constant__ CUtensorMap tmap_dy,
+                           const __grid_constant__ CUtensorMap tmap_x) {
+  using Cfg = WgradSmallCfg<IMG>;
+  constexpr int NS = Cfg::NS, STAGE = Cfg::STAGE, NCO = kWgradSmallCols;
+  extern __shared__ __align__(16) uint8_t smem_raw[];
+  __shared__ __align__(8) uint64_t full_bar[NS], empty_bar[NS];
+  const uint32_t sbase = (smem_u32(smem_raw) + 1023u) & ~1023u;
+  const int tid = threadIdx.x, wg_id = tid >> 7, t = tid & 127;
+  const int nci = (a.Ci + 63) / 64;
+  const int s_tap = blockIdx.y % 3, cb = (blockIdx.y / 3) % nci, nb = blockIdx.y / (3 * nci);
   if (tid == 0) {
 #pragma unroll
-    for (int i = 0; i < NST; ++i) mbar_init(&dy_bar[i], 1);
+    for (int i = 0; i < NS; ++i) {
+      mbar_init(&full_bar[i], 1);
+      mbar_init(&empty_bar[i], 3);   // one arrival per consumer warpgroup
+    }
     mbar_fence_init();
   }
-  // rows beyond the loaded ones are read by the (discarded) padding M rows: keep them finite
-  for (int st = 0; st < NST; ++st)
-    for (int v = tid; v < (HROWS_A - HROWS_LOAD) * RP / 16; v += 128) {
-      const uint32_t addr = sbase + st * STAGE + HROWS_LOAD * RP + v * 16;
-      asm volatile("st.shared.v4.b32 [%0], {%1,%1,%1,%1};" ::"r"(addr), "r"(0u) : "memory");
-    }
-  // Operand traffic.  In an all-cp.async version every LDGSTS of the dy tile costs 64 shared-memory wavefronts
-  // (ideal 8) -- a 16-byte copy only coalesces with its neighbours when 8 lanes are contiguous in BOTH global and
-  // shared memory, and the MN-major no-swizzle layout ([channel chunk][pixel][16 B]) is a transpose of the pixel-major
-  // tensor; 5700 LSU cycles per tile against 1536 tensor cycles.  The dy tile now arrives by TMA (box = 64 channels x
-  // 8 x IMG x IPT pixels, hardware 128-byte swizzle = the MN-major SWIZZLE_128B operand layout; for 4x4 images the box
-  // is 8 wide and the 4 out-of-range columns are the zero "virtual pixels"): zero LSU work, one thread.  Warps 1-3
-  // keep loading the x halo with cp.async (its shifted-descriptor layout has no TMA box form).
-  // x halo: LDG.128 into registers (4 lanes = the 64 bytes of one pixel's channel slice, consecutive pixels follow),
-  // later STS.128 into the shifted-descriptor layout -- 8x fewer LSU cycles than the same copies as LDGSTS
-  constexpr int XV = HROWS_LOAD * CJ * HWD, XPER = (XV + 95) / 96;
-  uint4 xr[XPER];
-  auto fetch_x = [&](int tile) {
-    if (warp == 0) return;
-    const int lt = tid - 32;
-    const int b0 = tile * IPT;
-#pragma unroll
-    for (int i = 0; i < XPER; ++i) {
-      const int v = lt + i * 96;
-      uint4 r = make_uint4(0u, 0u, 0u, 0u);
-      if (v < XV) {
-        const int cj = v % CJ;
-        const int t = v / CJ;
-        const int hx = t % HWD, hy = t / HWD;
-        const int j = hy / RPI, ih = hy - j * RPI - 1, iw = hx - 1;
-        const int b = b0 + j;
-        if (b < a.B && ih >= 0 && ih < IMG && iw >= 0 && iw < IMG)
-          r = __ldg(reinterpret_cast<const uint4*>(a.x + ((((size_t)b * IMG + ih) * IMG + iw) * a.Ci + c_off + cj * 8)));
-      }
-      xr[i] = r;
-    }
-  };
-  auto store_x = [&](int st) {
-    if (warp == 0) return;
-    const int lt = tid - 32;
-    const uint32_t sh = sbase + st * STAGE;
-#pragma unroll
-    for (int i = 0; i < XPER; ++i) {
-      const int v = lt + i * 96;
-      if (v < XV) {
-        const int cj = v % CJ;
-        const int t = v / CJ;
-        const int hx = t % HWD, hy = t / HWD;
-        asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(sh + (uint32_t)(((hy * CJ + cj) * HWD + hx) * 16)),
-                     "r"(xr[i].x), "r"(xr[i].y), "r"(xr[i].z), "r"(xr[i].w) : "memory");
-      }
-    }
-  };
-  auto load_dy = [&, tmap_p](int tile, int st) {   // thread 0 only
-    const uint32_t sd = sbase + st * STAGE + HALO_BYTES;
-    mbar_expect_tx(&dy_bar[st], (uint32_t)DY_BYTES);
-#pragma unroll
-    for (int nb = 0; nb < NB; ++nb)
-      tma_load_4d(sd + (uint32_t)nb * (128 * 128), tmap_p, &dy_bar[st], n_off + nb * 64, 0, 0, tile * IPT);
-  };
+  if (tid < NS * 8)   // the first 128 bytes of every stage's gap
+    asm volatile("st.shared.v4.b32 [%0], {%1,%1,%1,%1};" ::"r"(sbase + (tid / 8) * STAGE + Cfg::DYB + Cfg::XB + (tid % 8) * 16),
+                 "r"(0u) : "memory");
+  fence_proxy_async_smem();   // st.shared (generic proxy) -> wgmma reads (async proxy)
+  __syncthreads();
   const int first = blockIdx.x, stride = gridDim.x;
   const int my_n = first < a.ntiles ? (a.ntiles - first + stride - 1) / stride : 0;
-  // prologue: tiles 0 .. NST-2 staged
-#pragma unroll
-  for (int i = 0; i < NST - 1; ++i) {
-    if (i < my_n) {
-      fetch_x(first + i * stride);
-      store_x(i);
-      if (tid == 0) load_dy(first + i * stride, i);
-    }
-  }
-  fence_proxy_async_smem();
-  __syncthreads();
-  float acc_t[NS];
 
-  for (int it = 0; it < my_n; ++it) {
-    const int st = it % NST;
-    const int nt = it + NST - 1;     // the tile that will refill the stage tile it-1 used
-    if (nt < my_n) fetch_x(first + nt * stride);   // its x halo: global loads in flight from here on
-    fence_proxy_async_smem();        // x halo of tile it was stored (st.shared) an iteration ago
-    __syncthreads();
-    mbar_wait(&dy_bar[st], (it / NST) & 1);   // the TMA'd dy tile
-    {
-      const uint32_t sh = sbase + st * STAGE;
-      const uint32_t sd = sh + HALO_BYTES;
+  if (wg_id == 3) {
+    if (t == 0) {
+      const CUtensorMap* const pd = &tmap_dy;   // param-space addresses, taken in the kernel body
+      const CUtensorMap* const px = &tmap_x;
+      for (int it = 0; it < my_n; ++it) {
+        const int st = it % NS;
+        if (it >= NS) mbar_wait(&empty_bar[st], ((it / NS) - 1) & 1);
+        const int b0 = (first + it * stride) * Cfg::NIMG;
+        const uint32_t sd = sbase + (uint32_t)st * STAGE;
+        mbar_expect_tx(&full_bar[st], (uint32_t)(Cfg::DYB + Cfg::XB));   // the gap is not loaded
+#pragma unroll
+        for (int j = 0; j < NCO / 64; ++j)
+          tma_load_4d(sd + (uint32_t)j * Cfg::DYBLK, pd, &full_bar[st], nb * NCO + j * 64, 0, 0, b0);
+        tma_load_5d(sd + Cfg::DYB, px, &full_bar[st], 0, s_tap - 1, -1, b0, cb * 8);
+      }
+    }
+  } else {
+    const int r = wg_id;   // vertical tap of this warpgroup's accumulator
+    float acc[NCO / 2];
+    for (int it = 0; it < my_n; ++it) {
+      const int st = it % NS;
+      mbar_wait(&full_bar[st], (it / NS) & 1);
+      const uint32_t sd = sbase + (uint32_t)st * STAGE, sx = sd + Cfg::DYB;
       wgmma_fence();
 #pragma unroll
-      for (int ks = 0; ks < TH / 2; ++ks) {
-        // K16 = tile rows 2ks, 2ks+1 (never straddle an image: IMG is even) -> halo rows hb, hb+1 (+ tap r in M)
-        const int hb = ((2 * ks) / IMG) * RPI + (2 * ks) % IMG;
-        const uint64_t da = make_smem_desc(sh + hb * RP + s_tap * 16, RP, P, kNoSwizzle);
-        // B: MN-major, 128-byte swizzle: rows = pixels (K), 128 B = 64 channels; K16 = 2 groups of 8 rows (1024 B each);
-        // LBO = next 64-channel block (128 rows x 128 B), SBO = next 8-row group
-        const uint64_t db = make_smem_desc(sd + ks * 2048, 128 * 128, 1024, kSwizzle128B);
-        mma128<NS, kBF16, 1, 1>(acc_t, da, 8 * P, db, (it > 0 || ks > 0) ? 1u : 0u);
+      for (int k = 0; k < TH / 2; ++k) {
+        // tile rows 2k, 2k+1 = image j, output rows oh0, oh0 + 1 (IMG is even: never straddles an image); tap r = r
+        // rows further down
+        const int j = (2 * k) / IMG, oh0 = (2 * k) % IMG;
+        const uint64_t da = make_smem_desc(sx + (uint32_t)((j * (IMG + 2) + oh0 + r) * Cfg::ROWB), Cfg::ROWB, Cfg::CHUNK,
+                                           kNoSwizzle);
+        // B: MN-major, 128-byte swizzle: K16 = 2 groups of 8 pixel rows (SBO 1024 B), LBO = next 64-channel block
+        const uint64_t db = make_smem_desc(sd + (uint32_t)k * 2048, Cfg::DYBLK, 1024, kSwizzle128B);
+        Wgmma<NCO, kBF16>::template mma<1, 1>(acc, da, db, (it > 0 || k > 0) ? 1u : 0u);
       }
       wgmma_commit();
-      wgmma_wait<0>();
+      wgmma_wait<1>();   // the MMAs of tile it-1 have read their stage: release it to the producer
+      if (it > 0 && t == 0) mbar_arrive(&empty_bar[(it - 1) % NS]);
     }
-    // refill the stage tile it-1 used (its MMAs are complete) with tile it+NST-1
-    if (nt < my_n) {
-      store_x(nt % NST);
-      if (tid == 0) load_dy(first + nt * stride, nt % NST);
+    wgmma_wait<0>();
+    if (my_n == 0) {   // a worker without tiles still writes its (zero) partial
+#pragma unroll
+      for (int i = 0; i < NCO / 2; ++i) acc[i] = 0.f;
     }
-  }
-  {   // a worker without tiles still writes its (zero) partial
-    if (my_n == 0) {
+    acc_fence(acc);
+    // fragment: rows 16w + l/4 (+8), columns 8i + 2(l%4) (+1); 4 lanes write one 32-byte sector
+    const int w = t >> 5, l = t & 31;
+    const int ci = cb * 64 + 16 * w + (l >> 2);
+    float* const dst = a.dw + ((size_t)blockIdx.x * 9 * a.Ci + (size_t)(r * 3 + s_tap) * a.Ci + ci) * a.Co +
+                       nb * NCO + 2 * (l & 3);
 #pragma unroll
-      for (int j = 0; j < NS; ++j) acc_t[j] = 0.f;
-    }
-    acc_fence(acc_t);
-    const int blk = tid >> 3;                  // row block (r, cj)
-    const int r = blk / CJ, cj = blk % CJ;
-    const bool ok = r < KH;
-    const size_t row = (size_t)(r * KW + s_tap) * a.Ci + c_off + cj * 8 + (tid & 7);
+    for (int h = 0; h < 2; ++h) {
+      if (ci + 8 * h < a.Ci) {
 #pragma unroll
-    for (int col0 = 0; col0 < NS; col0 += 32) {
-      float rr[32];
-      acc_row32(acc_t, col0, stage_buf, rr);
-      if (ok) {
-        float* dst = a.dw + ((size_t)blockIdx.x * 9 * a.Ci + row) * a.Co + n_off + col0;
-#pragma unroll
-        for (int j = 0; j < 32; j += 4) *reinterpret_cast<float4*>(dst + j) = make_float4(rr[j], rr[j + 1], rr[j + 2], rr[j + 3]);
+        for (int i = 0; i < NCO / 8; ++i)
+          *reinterpret_cast<float2*>(dst + (size_t)(8 * h) * a.Co + 8 * i) = make_float2(acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1]);
       }
     }
   }
@@ -1176,12 +1140,12 @@ static EncodeTiledFn halo_encode_fn() {
   return fn;
 }
 
-static int blocks_per_sm(const void* kern, size_t smem, int* cache) {
+static int blocks_per_sm(const void* kern, size_t smem, int* cache, int threads = 128) {
   if (*cache > 0) return *cache;
   cudaFuncAttributes fa;
   if (cudaFuncGetAttributes(&fa, kern) != cudaSuccess) return 1;
   const int regs = fa.numRegs > 0 ? fa.numRegs : 128;
-  int by_regs = 65536 / (((regs + 7) / 8 * 8) * 128);
+  int by_regs = 65536 / (((regs + 7) / 8 * 8) * threads);
   int by_smem = (int)((227 * 1024) / (smem + fa.sharedSizeBytes + 1024));
   int n = by_regs < by_smem ? by_regs : by_smem;
   if (n > 16) n = 16;
@@ -1393,55 +1357,62 @@ static int launch_halo_wgrad(const HaloWgradArgs& a, cudaStream_t st) {
   return reduce_partials(parts, grid, count, count, a.dw, parts + (size_t)grid * count, st);
 }
 
-template <int NS, int IMG>
-static int launch_halo_wgrad_small(const HaloWgradSmallArgs& a, cudaStream_t st) {
-  constexpr int RP = 4 * (TW + 2) * 16, IPT = TH / IMG, RPI = IMG + 2;
-  constexpr int HROWS_LOAD = IPT * RPI, HROWS = (IPT - 1) * RPI + (IMG - 2) + 1 + 4;
-  constexpr int HROWS_A = HROWS > HROWS_LOAD ? HROWS : HROWS_LOAD;
-  constexpr int HALO_BYTES = (HROWS_A * RP + 1023) / 1024 * 1024;
-  const size_t smem = kSmallWgradStages * (size_t)(HALO_BYTES + (NS / 64) * 128 * 128) + 1024 + 64;
+template <int IMG>
+static int launch_wgrad_small(const grad_t* x, const grad_t* dy, float* dw, int B, int Ci, int Co, cudaStream_t st) {
+  using Cfg = WgradSmallCfg<IMG>;
   EncodeTiledFn enc = halo_encode_fn();
   if (!enc) {
     set_last_error("conv_halo_wgrad (small images): cuTensorMapEncodeTiled is not available from this driver");
     return HB200_ERR_UNSUPPORTED;
   }
-  // dy bf16 [B, IMG, IMG, Co]: box = 64 channels (one 128-byte swizzled row per pixel) x 8 columns x IMG rows x IPT images;
-  // columns / images past the tensor are zero-filled (the virtual pixels of 4x4 images, the ragged last tile)
-  CUtensorMap tmap;
-  const cuuint64_t dims[4] = {(cuuint64_t)a.Co, (cuuint64_t)IMG, (cuuint64_t)IMG, (cuuint64_t)a.B};
-  const cuuint64_t strides[3] = {(cuuint64_t)a.Co * 2, (cuuint64_t)IMG * a.Co * 2, (cuuint64_t)IMG * IMG * a.Co * 2};
-  const cuuint32_t box[4] = {64u, 8u, (cuuint32_t)IMG, (cuuint32_t)IPT};
-  const cuuint32_t estr[4] = {1u, 1u, 1u, 1u};
-  const CUresult r = enc(&tmap, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, (void*)a.dy, dims, strides, box, estr,
-                         CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  // dy bf16 [B, IMG, IMG, Co]: box = 64 channels (one 128-byte swizzled row per pixel) x 8 columns x IMG rows x the
+  // stage's images; columns / frames past the tensor are zero-filled (4x4 images, the ragged last tile)
+  CUtensorMap tmap_dy, tmap_x;
+  const cuuint64_t dims[4] = {(cuuint64_t)Co, (cuuint64_t)IMG, (cuuint64_t)IMG, (cuuint64_t)B};
+  const cuuint64_t strides[3] = {(cuuint64_t)Co * 2, (cuuint64_t)IMG * Co * 2, (cuuint64_t)IMG * IMG * Co * 2};
+  const cuuint32_t box[4] = {64u, (cuuint32_t)TW, (cuuint32_t)IMG, (cuuint32_t)Cfg::NIMG};
+  const cuuint32_t estr[5] = {1u, 1u, 1u, 1u, 1u};
+  CUresult r = enc(&tmap_dy, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, (void*)dy, dims, strides, box, estr,
+                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
-    set_last_error("conv_halo_wgrad (small images): cuTensorMapEncodeTiled failed (%d)", (int)r);
+    set_last_error("conv_halo_wgrad (small images): cuTensorMapEncodeTiled (dy) failed (%d)", (int)r);
     return HB200_ERR_CUDA;
   }
-  auto kern = conv_halo_wgrad_small_kernel<NS, IMG>;
-  static bool attr = false;
-  if (!attr) {
-    HB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    attr = true;
+  // x bf16 [B, IMG, IMG, Ci] seen as (8 ch | column | row | frame | chunk): box = 8 ch x IMG columns x IMG + 2 rows x
+  // the stage's images x 8 chunks, i.e. [chunk][image][padded row][pixel][8 ch] in shared memory
+  const cuuint64_t xd[5] = {8u, (cuuint64_t)IMG, (cuuint64_t)IMG, (cuuint64_t)B, (cuuint64_t)(Ci / 8)};
+  const cuuint64_t xs[4] = {(cuuint64_t)Ci * 2, (cuuint64_t)IMG * Ci * 2, (cuuint64_t)IMG * IMG * Ci * 2, 16u};
+  const cuuint32_t xb[5] = {8u, (cuuint32_t)IMG, (cuuint32_t)(IMG + 2), (cuuint32_t)Cfg::NIMG, 8u};
+  r = enc(&tmap_x, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 5, (void*)x, xd, xs, xb, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+          CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) {
+    set_last_error("conv_halo_wgrad (small images): cuTensorMapEncodeTiled (x) failed (%d)", (int)r);
+    return HB200_ERR_CUDA;
   }
-  const int slices = (a.Ci / 32) * (a.Co / NS) * 3;   // channel slices x the 3 horizontal taps (one accumulator each)
-  int workers = 2 * kNumSMs / slices;
+  auto kern = conv_wgrad_small_ws_kernel<IMG>;
+  static int cache = 0;
+  if (cache == 0) HB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Cfg::SMEM));
+  // the grid is sized from the CTAs that fit per SM (registers of 416 threads, the stage ring): one here
+  const int per_sm = blocks_per_sm((const void*)kern, Cfg::SMEM, &cache, kWgradSmallThreads);
+  const int ntiles = (B + Cfg::NIMG - 1) / Cfg::NIMG;
+  const int slices = (Ci + 63) / 64 * 3 * (Co / kWgradSmallCols);   // (ci block, horizontal tap, co block)
+  int workers = kNumSMs * per_sm / slices;
   if (workers < 1) workers = 1;
-  if (workers > a.ntiles) workers = a.ntiles;
+  if (workers > ntiles) workers = ntiles;
   // one partial per worker, summed in worker order into the caller's accumulator (deterministic)
-  const long long count = 9LL * a.Ci * a.Co;
+  const long long count = 9LL * Ci * Co;
   float* parts = nullptr;
   int* tickets = nullptr;
   int rc = stream_workspace(st, (size_t)(workers + (workers < kReduceChunks ? workers : kReduceChunks)) * count, 0, &parts,
                             &tickets);
   if (rc) return rc;
-  HaloWgradSmallArgs ap = a;
-  ap.dw = parts;
-  kern<<<dim3(workers, slices), 128, smem, st>>>(ap, tmap);
+  WgradSmallArgs a;
+  a.dw = parts; a.Ci = Ci; a.Co = Co; a.ntiles = ntiles;
+  kern<<<dim3(workers, slices), kWgradSmallThreads, Cfg::SMEM, st>>>(a, tmap_dy, tmap_x);
   HB_LAUNCH_OK();
   count_launch(1);
-  return reduce_partials(parts, workers, count, count, a.dw, parts + (size_t)workers * count, st);
+  return reduce_partials(parts, workers, count, count, dw, parts + (size_t)workers * count, st);
 }
 }  // namespace hb200
 
@@ -1464,7 +1435,7 @@ extern "C" int hb200_conv_halo_supported(int c, int n, int k, int h, int w) {
   return 0;
 }
 
-/* weight-gradient variant: additionally the small-image layers (8x8 / 4x4, channels sliced 32 x 128) */
+/* weight-gradient variant: additionally the small-image layers (8x8 / 4x4, channels sliced 64 x 128) */
 extern "C" int hb200_conv_halo_wgrad_supported(int c, int n, int k, int h, int w) {
   if (hb200_conv_halo_supported(c, n, k, h, w)) return 1;
   return k == 3 && c % 32 == 0 && n % 128 == 0 && h == w && (h == 8 || h == 4);
@@ -1580,13 +1551,11 @@ extern "C" int hb200_conv_halo_wgrad(const hb200_bf16* x, const hb200_bf16* dy, 
                                      int w, int c, int n, int k, hb200_stream_t stream) {
   HB_CHECK_ARG(x && dy && dw_acc, "conv_halo_wgrad: null pointer");
   HB_CHECK_ARG(hb200_conv_halo_wgrad_supported(c, n, k, h, w), "conv_halo_wgrad: unsupported shape C=%d N=%d k=%d %dx%d", c, n, k, h, w);
-  if (!hb200_conv_halo_supported(c, n, k, h, w)) {   // small images: several images per tile, sliced channels
-    HaloWgradSmallArgs s;
-    s.x = (const grad_t*)x; s.dy = (const grad_t*)dy; s.dw = dw_acc;
-    s.B = batch; s.Ci = c; s.Co = n;
-    const int ipt = TH / h;
-    s.ntiles = (batch + ipt - 1) / ipt;
-    return h == 8 ? launch_halo_wgrad_small<128, 8>(s, (cudaStream_t)stream) : launch_halo_wgrad_small<128, 4>(s, (cudaStream_t)stream);
+  if (!hb200_conv_halo_supported(c, n, k, h, w)) {   // small images: 16x8 tiles of stacked images, sliced channels
+    const grad_t* xg = (const grad_t*)x;
+    const grad_t* dyg = (const grad_t*)dy;
+    cudaStream_t st = (cudaStream_t)stream;
+    return h == 8 ? launch_wgrad_small<8>(xg, dyg, dw_acc, batch, c, n, st) : launch_wgrad_small<4>(xg, dyg, dw_acc, batch, c, n, st);
   }
   HaloWgradArgs a;
   a.x = (const __nv_bfloat16*)x; a.dy = (const __nv_bfloat16*)dy; a.dw = dw_acc;

@@ -47,22 +47,12 @@ SIGNATURES = {
     "hb200_pack_conv_weight": ("i", "ppp" + "iiiii" + "p"),
     "hb200_unpack_conv_wgrad": ("i", "pp" + "iiiii" + "p"),
     "hb200_packed_weight_elems": ("z", "iiii"),
-    "hb200_set_umma_layout": ("i", "i"),
-    "hb200_get_umma_layout": ("i", ""),
-    "hb200_set_halo_tma": ("i", "i"),
-    "hb200_get_halo_tma": ("i", ""),
     "hb200_conv_s2_supported": ("i", "iiiii"),
-    "hb200_set_conv_s2_ws": ("i", "i"),
-    "hb200_get_conv_s2_ws": ("i", ""),
     "hb200_conv_s2_wgrad_supported": ("i", "iiii"),
     "hb200_conv_s2_wgrad": ("i", "ppp" + "iiiii" + "p"),
     "hb200_unpack_s2_wgrad": ("i", "pp" + "ii" + "p"),
     "hb200_conv_s2_fwd": ("i", "pppp" + "pipi" + "iiiiii" + "p"),
     "hb200_conv_s2_dgrad": ("i", "ppppp" + "iiiiii" + "p"),
-    "hb200_set_wgrad_xtma": ("i", "i"),
-    "hb200_get_wgrad_xtma": ("i", ""),
-    "hb200_set_tgemm_tma": ("i", "i"),
-    "hb200_get_tgemm_tma": ("i", ""),
     "hb200_conv_halo_supported": ("i", "iiiii"),
     "hb200_conv_halo_wgrad_supported": ("i", "iiiii"),
     "hb200_pack_halo_weight": ("i", "pp" + "iiiiii" + "p"),

@@ -12,10 +12,10 @@
 //   wgrad   : D[(r,s,ci), co] = sum_{pixel}  X[pixel@(r,s), ci] * dY[pixel, co]     (MN-major,
 //             split over pixel slabs, fp32 atomics into the accumulator)
 //
-// Shared-memory operand layouts (selected at runtime, pinned by hb200_umma_gemm_probe):
-//   layout 0: no-swizzle "interleaved" core matrices: 16-byte vector (row, k8) at
-//             k8 * rows*16 + row*16               (LBO = rows*16, SBO = 128)
-//   layout 1: 128-byte swizzle: (row>>3)*1024 + (row&7)*128 + ((k8 ^ (row&7)) << 4)
+// Shared-memory operand layout of the conv kernels and their weight images (128-byte swizzle, K-major): 16-byte vector
+// (row, k8) at (row>>3)*1024 + (row&7)*128 + ((k8 ^ (row&7)) << 4).  hb200_umma_gemm_probe pins it on hardware, together
+// with the no-swizzle descriptor forms the halo kernels use (probe layout 0: "interleaved" core matrices, vector (row, k8)
+// at k8 * rows*16 + row*16, LBO = rows*16, SBO = 128).
 #include <cuda.h>
 
 #include "common.cuh"
@@ -23,7 +23,6 @@
 
 namespace hb200 {
 void count_launch(int n);
-static int g_umma_layout = 1;  // 128-byte swizzle (coalesced gathers); 0 = no-swizzle interleave
 
 using namespace wg;
 
@@ -66,7 +65,7 @@ struct ConvArgs {
 
 // NST = depth of the cp.async ring.  3 at the learner's sizes (several CTAs per SM hide the latency); the few-CTA launches
 // of the actor are one dependent memory latency per chunk and get a deeper ring instead.
-template <int BN, int MODE, int LAYOUT, int NST = kStages>
+template <int BN, int MODE, int NST>
 __global__ void __launch_bounds__(128) conv_igemm_kernel(const ConvArgs a) {
   extern __shared__ __align__(16) uint8_t smem_raw[];
   constexpr uint32_t kABytes = kTileM * kChunkK * 2;
@@ -113,11 +112,11 @@ __global__ void __launch_bounds__(128) conv_igemm_kernel(const ConvArgs a) {
     op = rem / a.OW;
     oq = rem - op * a.OW;
   }
-  // LAYOUT 1 (128-byte swizzle) gathers with a coalesced mapping -- 8 consecutive lanes fetch the 8 x 16 B of ONE
+  // The 128-byte-swizzle layout gathers with a coalesced mapping -- 8 consecutive lanes fetch the 8 x 16 B of ONE
   // pixel's 64-channel run (one full 128-byte line) and write one swizzled smem row -- so every thread needs the
   // pixel coordinates of 8 other rows: publish them once per tile.
   __shared__ int4 row_info[kTileM];
-  if (LAYOUT == 1) row_info[tid] = make_int4(ob, op, oq, row_ok ? 1 : 0);
+  row_info[tid] = make_int4(ob, op, oq, row_ok ? 1 : 0);
   if (tid == 0) {
     int nv = 0;
     const int cpt = a.SC >> 6;  // 64-channel chunks per tap (>= 1 in class mode)
@@ -142,88 +141,60 @@ __global__ void __launch_bounds__(128) conv_igemm_kernel(const ConvArgs a) {
   const __nv_bfloat16* wtile =
       a.wimg + (size_t)(n0 / wbn) * a.nchunks * ((size_t)wbn * kChunkK) + (size_t)(n0 % wbn) * kChunkK;
 
-  // LAYOUT 1: the 8 rows this thread gathers for (row = tid/8 + 16 i) never change -> their pixel origin lives in
+  // The 8 rows this thread gathers for (row = tid/8 + 16 i) never change -> their pixel origin lives in
   // registers (frame base, first input row / column of the window; an out-of-range row gets an origin no tap can reach).
   // Per chunk and row that leaves two adds, two unsigned range checks and the address (this loop was 440 warp
   // instructions per chunk and the whole cost of the few-CTA launches, where one warp per scheduler hides nothing).
   int rbase[8], rh[8], rw[8];
   uint32_t soff[8];
   const int jv = tid & 7;
-  if (LAYOUT == 1) {
 #pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      const int row = (tid >> 3) + 16 * i;
-      const int4 ri = row_info[row];
-      rbase[i] = ri.x * a.SH * a.SW;
-      if (MODE == 0) {
-        rh[i] = ri.w ? ri.y * a.stride - a.pad : -(1 << 20);
-        rw[i] = ri.z * a.stride - a.pad;
-      } else {
-        rh[i] = ri.w ? ri.y + a.pad : -(1 << 20);
-        rw[i] = ri.z + a.pad;
-      }
-      soff[i] = tile_off<1>(row, jv, kTileM);
+  for (int i = 0; i < 8; ++i) {
+    const int row = (tid >> 3) + 16 * i;
+    const int4 ri = row_info[row];
+    rbase[i] = ri.x * a.SH * a.SW;
+    if (MODE == 0) {
+      rh[i] = ri.w ? ri.y * a.stride - a.pad : -(1 << 20);
+      rw[i] = ri.z * a.stride - a.pad;
+    } else {
+      rh[i] = ri.w ? ri.y + a.pad : -(1 << 20);
+      rw[i] = ri.z + a.pad;
     }
+    soff[i] = tile_off<1>(row, jv, kTileM);
   }
   const int inv_kw = 65536 / a.kw + 1;   // tap / kw == (tap * inv_kw) >> 16 for tap < 8192, kw <= 8
 
   auto load_chunk = [&](int chunk, int stage) {
     const uint32_t sa = smem_base + stage * kStageBytes;
     const uint32_t sb = sa + kABytes;
-    if (LAYOUT == 1) {
-      const int k0 = (chunk * 8 + jv) << 3;
-      const int tap = k0 >> a.cshift;
-      const int c0 = k0 & (a.SC - 1);
-      const int r = (tap * inv_kw) >> 16, s = tap - r * a.kw;
-      const bool tap_ok = tap < taps;
-      const __nv_bfloat16* srcc = a.src + c0;
+    const int k0 = (chunk * 8 + jv) << 3;
+    const int tap = k0 >> a.cshift;
+    const int c0 = k0 & (a.SC - 1);
+    const int r = (tap * inv_kw) >> 16, s = tap - r * a.kw;
+    const bool tap_ok = tap < taps;
+    const __nv_bfloat16* srcc = a.src + c0;
 #pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        int ih, iw;
-        bool ok = tap_ok;
-        if (MODE == 0) {
-          ih = rh[i] + r;
-          iw = rw[i] + s;
-        } else {
-          const int th = rh[i] - r, tw = rw[i] - s;
-          if (a.stride == 1) {
-            ih = th; iw = tw;
-          } else if (a.stride == 2) {
-            ih = th >> 1; iw = tw >> 1;
-            ok = ok && (((th | tw) & 1) == 0);
-          } else {
-            ih = th / a.stride; iw = tw / a.stride;
-            ok = ok && th >= 0 && tw >= 0 && (ih * a.stride == th) && (iw * a.stride == tw);
-          }
-        }
-        ok = ok && (unsigned)ih < (unsigned)a.SH && (unsigned)iw < (unsigned)a.SW;
-        const __nv_bfloat16* g = ok ? srcc + ((size_t)(rbase[i] + ih * a.SW + iw) << a.cshift) : a.src;
-        cp_async16(sa + soff[i], g, ok);
-      }
-    } else {
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      const int k0 = (chunk * 8 + j) << 3;
-      const int tap = k0 >> a.cshift;
-      const int c0 = k0 & (a.SC - 1);
-      const int r = tap / a.kw, s = tap - r * a.kw;
-      bool ok = row_ok && tap < taps;
+    for (int i = 0; i < 8; ++i) {
       int ih, iw;
+      bool ok = tap_ok;
       if (MODE == 0) {
-        ih = op * a.stride - a.pad + r;
-        iw = oq * a.stride - a.pad + s;
-        ok = ok && ih >= 0 && ih < a.SH && iw >= 0 && iw < a.SW;
+        ih = rh[i] + r;
+        iw = rw[i] + s;
       } else {
-        const int th = op + a.pad - r, tw = oq + a.pad - s;
-        ih = th / a.stride;
-        iw = tw / a.stride;
-        ok = ok && th >= 0 && tw >= 0 && (ih * a.stride == th) && (iw * a.stride == tw) &&
-             ih < a.SH && iw < a.SW;
+        const int th = rh[i] - r, tw = rw[i] - s;
+        if (a.stride == 1) {
+          ih = th; iw = tw;
+        } else if (a.stride == 2) {
+          ih = th >> 1; iw = tw >> 1;
+          ok = ok && (((th | tw) & 1) == 0);
+        } else {
+          ih = th / a.stride; iw = tw / a.stride;
+          ok = ok && th >= 0 && tw >= 0 && (ih * a.stride == th) && (iw * a.stride == tw);
+        }
       }
-      const __nv_bfloat16* g =
-          ok ? a.src + ((((size_t)ob * a.SH + ih) * a.SW + iw) << a.cshift) + c0 : a.src;
-      cp_async16(sa + tile_off<LAYOUT>(tid, j, kTileM), g, ok);
-    }
+      ok = ok && (unsigned)ih < (unsigned)a.SH && (unsigned)iw < (unsigned)a.SW;
+      const __nv_bfloat16* g = ok ? srcc + ((size_t)(rbase[i] + ih * a.SW + iw) << a.cshift) : a.src;
+      cp_async16(sa + soff[i], g, ok);
     }
     const uint4* wsrc = reinterpret_cast<const uint4*>(wtile + (size_t)chunk * ((size_t)wbn * kChunkK));
 #pragma unroll
@@ -253,7 +224,7 @@ __global__ void __launch_bounds__(128) conv_igemm_kernel(const ConvArgs a) {
       wgmma_fence();
 #pragma unroll
       for (int kk = 0; kk < kChunkK / 16; ++kk)
-        mma128<BN, kT>(acc_t, kmajor_desc<LAYOUT>(sa, kk, kTileM), kmajor_hi<LAYOUT>(), kmajor_desc<LAYOUT>(sb, kk, BN),
+        mma128<BN, kT>(acc_t, kmajor_desc<1>(sa, kk, kTileM), kmajor_hi<1>(), kmajor_desc<1>(sb, kk, BN),
                        (c > 0 || kk > 0) ? 1u : 0u);
       wgmma_commit();
     }
@@ -375,8 +346,8 @@ __global__ void __launch_bounds__(128) conv_igemm_kernel(const ConvArgs a) {
 // (address arithmetic and predicates for 8 rows per thread per chunk) between its MMAs, and its 128 x 128 tile reads
 // 32 KB from L2 per 2.1 MFLOP.  Here:
 //   warpgroup 0 (one thread)  producer: per K chunk (one filter tap x 64 channels) one TMA im2col box of the activation
-//                             (forward) or gradient (dgrad) in the 128-byte-swizzle K-major layout (LAYOUT 1, byte for
-//                             byte what the gather writes; padding is the TMA unit's zero fill) and one 16 KB bulk copy
+//                             (forward) or gradient (dgrad) in the 128-byte-swizzle K-major layout (byte for byte
+//                             what the gather kernel writes; padding is the TMA unit's zero fill) and one 16 KB bulk copy
 //                             per 128 columns of the packed weight image, into a kWsStages-deep full / empty mbarrier ring
 //   warpgroups 1, 2           consumers: both work on the same CTA tile and read the same stage, each with a 128 x 128
 //                             fp32 accumulator.  SPLIT_N = false: tile 256 pixels x 128 channels, the consumers split M
@@ -810,7 +781,7 @@ umma_probe_kernel(const __nv_bfloat16* __restrict__ A, const __nv_bfloat16* __re
 __global__ void pack_weight_kernel(const float* __restrict__ w, __nv_bfloat16* __restrict__ img,
                                    int rows /*N dim*/, int BN, int kc /*channels per tap*/,
                                    int kc_real, int taps, int kw, int nchunks, int transposed,
-                                   int co, int ci_real, int layout) {
+                                   int co, int ci_real) {
   // one thread per 16-byte vector of the image
   const long long nvec = (long long)(rows / BN) * nchunks * BN * 8;
   for (long long v = blockIdx.x * (long long)blockDim.x + threadIdx.x; v < nvec;
@@ -819,16 +790,9 @@ __global__ void pack_weight_kernel(const float* __restrict__ w, __nv_bfloat16* _
     const long long t = v / per_tile;
     const int within = (int)(v - t * per_tile);
     const int ntile = (int)(t / nchunks), chunk = (int)(t - (long long)ntile * nchunks);
-    // invert the layout: find (row, k8) stored at vector slot `within`
-    int row, k8;
-    if (layout == 0) {
-      k8 = within / BN;
-      row = within - k8 * BN;
-    } else {
-      const int g = within >> 6, rr = (within >> 3) & 7, pos = within & 7;
-      row = g * 8 + rr;
-      k8 = pos ^ rr;
-    }
+    // invert the 128-byte swizzle: find (row, k8) stored at vector slot `within`
+    const int g = within >> 6, rr = (within >> 3) & 7, pos = within & 7;
+    const int row = g * 8 + rr, k8 = pos ^ rr;
     const int n = ntile * BN + row;
     float f[8];
 #pragma unroll
@@ -953,35 +917,31 @@ static int launch_igemm(ConvArgs a, int BN, cudaStream_t st) {
   // SM.  The gather kernel keeps the actor's few-tile launches, narrow gathers and stride 2: the dgrad has its parity
   // classes, and the stride-2 forwards (layer3 / layer4 entries) measured no faster on the im2col variant (it supports
   // them: element strides = the stride)
-  if (g_umma_layout == 1 && BN == kMaxBN && a.SC % kChunkK == 0 && !a.s2_classes && a.stride == 1 &&
+  if (BN == kMaxBN && a.SC % kChunkK == 0 && !a.s2_classes && a.stride == 1 &&
       a.bias == nullptr && !a.relu && 2LL * cdiv(a.M, kTileM) * (a.OC / kMaxBN) > kNumSMs) {
     if (a.OC >= 2 * kMaxBN) return launch_igemm_ws<MODE, true>(a, st);
     return launch_igemm_ws<MODE, false>(a, st);
   }
   // few output rows (the actor's 64-frame batches: 8 row tiles for the 4x4 layers): a 128-wide N tile leaves 16 CTAs on
-  // 132 SMs, each walking the whole K serially.  Narrower N tiles (slices of the packed tile, 128B-swizzle layout
-  // only) multiply the CTA count; the activation rows are re-gathered per slice out of L2.
-  bool deep = false;
-  if (g_umma_layout == 1) {
-    const int mt = a.s2_classes ? 4 * cdiv(a.M / 4, kTileM) : cdiv(a.M, kTileM);
-    while (BN > 32 && 2LL * mt * (a.OC / BN) <= kNumSMs) BN /= 2;
-    // at most one CTA per SM: nothing else hides the gather latency -> deep ring (uses the whole shared memory)
-    deep = (long long)mt * (a.OC / BN) <= kNumSMs && a.nchunks > kStages;
-  }
+  // 132 SMs, each walking the whole K serially.  Narrower N tiles (slices of the packed tile: whole 8-row groups of the
+  // 128B-swizzle layout) multiply the CTA count; the activation rows are re-gathered per slice out of L2.
+  const int mt = a.s2_classes ? 4 * cdiv(a.M / 4, kTileM) : cdiv(a.M, kTileM);
+  while (BN > 32 && 2LL * mt * (a.OC / BN) <= kNumSMs) BN /= 2;
+  // at most one CTA per SM: nothing else hides the gather latency -> deep ring (uses the whole shared memory)
+  const bool deep = (long long)mt * (a.OC / BN) <= kNumSMs && a.nchunks > kStages;
   // the kernel walks a per-CTA list of K chunks held in shared memory: a longer reduction must fail loudly, never truncate
   HB_CHECK_ARG(a.nchunks <= kMaxChunks, "conv: K = kh*kw*C = %d exceeds %d", a.nchunks * kChunkK, kMaxChunks * kChunkK);
   dim3 grid(a.s2_classes ? 4 * cdiv(a.M / 4, kTileM) : cdiv(a.M, kTileM), a.OC / BN);
-#define HB_CONV_CASE(bn, L, nst)                                                                \
+#define HB_CONV_CASE(bn, nst)                                                                   \
   {                                                                                             \
     const size_t smem = (size_t)(nst) * (kTileM * kChunkK * 2 + bn * kChunkK * 2) + 1024;       \
-    auto kern = conv_igemm_kernel<bn, MODE, L, nst>;                                            \
+    auto kern = conv_igemm_kernel<bn, MODE, nst>;                                               \
     HB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
     kern<<<grid, 128, smem, st>>>(a);                                                           \
   }
 #define HB_CONV_BN(bn, nst_deep)                                \
-  if (g_umma_layout == 0) HB_CONV_CASE(bn, 0, kStages)          \
-  else if (deep) HB_CONV_CASE(bn, 1, nst_deep)                  \
-  else HB_CONV_CASE(bn, 1, kStages)
+  if (deep) HB_CONV_CASE(bn, nst_deep)                          \
+  else HB_CONV_CASE(bn, kStages)
   switch (BN) {
     case 32: HB_CONV_BN(32, 8); break;
     case 64: HB_CONV_BN(64, 8); break;
@@ -1012,13 +972,6 @@ static int check_shape(const hb200_conv_shape* s) {
 }  // namespace hb200
 
 using namespace hb200;
-
-extern "C" int hb200_set_umma_layout(int layout) {
-  HB_CHECK_ARG(layout == 0 || layout == 1, "umma layout must be 0 or 1");
-  g_umma_layout = layout;
-  return HB200_OK;
-}
-extern "C" int hb200_get_umma_layout(void) { return g_umma_layout; }
 
 extern "C" int hb200_conv_fwd(const hb200_bf16* x, const hb200_bf16* w_packed, hb200_bf16* y,
                               double* gn_stats, int gn_groups, const hb200_conv_shape* s,
@@ -1153,8 +1106,7 @@ extern "C" int hb200_pack_conv_weight(const float* w_oihw, hb200_bf16* w_packed,
     const int BN = pick_bn(co), nchunks = cdiv((long long)taps * ci_pad, kChunkK);
     const long long nvec = (long long)(co / BN) * nchunks * BN * 8;
     pack_weight_kernel<<<(int)min((nvec + 255) / 256, (long long)kNumSMs * 8), 256, 0, st>>>(
-        w_oihw, (__nv_bfloat16*)w_packed, co, BN, ci_pad, ci_real, taps, kw, nchunks, 0, co, ci_real,
-        g_umma_layout);
+        w_oihw, (__nv_bfloat16*)w_packed, co, BN, ci_pad, ci_real, taps, kw, nchunks, 0, co, ci_real);
     HB_LAUNCH_OK();
     count_launch(1);
   }
@@ -1163,8 +1115,7 @@ extern "C" int hb200_pack_conv_weight(const float* w_oihw, hb200_bf16* w_packed,
     const int BN = pick_bn(ci_pad), nchunks = cdiv((long long)taps * co, kChunkK);
     const long long nvec = (long long)(ci_pad / BN) * nchunks * BN * 8;
     pack_weight_kernel<<<(int)min((nvec + 255) / 256, (long long)kNumSMs * 8), 256, 0, st>>>(
-        w_oihw, (__nv_bfloat16*)w_packed_t, ci_pad, BN, co, co, taps, kw, nchunks, 1, co, ci_real,
-        g_umma_layout);
+        w_oihw, (__nv_bfloat16*)w_packed_t, ci_pad, BN, co, co, taps, kw, nchunks, 1, co, ci_real);
     HB_LAUNCH_OK();
     count_launch(1);
   }

@@ -4,23 +4,20 @@
 //
 // The first-generation kernel (conv.cu) gathers an im2col tile per K chunk, so every input element
 // crosses L2 -> shared memory 9 times (L2-bound, the tensor pipe mostly idle).  Here each CTA loads the
-// (16+KH-1) x (8+KW-1) input halo of a 16x8 output tile ONCE into shared memory in the layout
+// (16+KH-1) x (8+KW-1) input halo of a 16x8 output tile ONCE into shared memory, and every filter tap is just a
+// different wgmma shared-memory descriptor over that one buffer (the forward / dgrad layouts are described at
+// conv_halo_ws_kernel).  The weight gradient stores the halo as
 //
 //        offset(hy, cj, hx) = ((hy * C/8 + cj) * HW + hx) * 16 bytes        (16 B = 8 channels)
 //
-// and every filter tap is just a different wgmma shared-memory descriptor over that one buffer:
-//   forward / dgrad (K-major A):  start = base + r*RP + s*16 + 2kk*P,  LBO = P (next 8 channels),
-//                                 SBO = RP (next output row = next 8-pixel core-matrix group)
-//   wgrad (MN-major A):           rows = (r, ci) with row-block stride P (because RP = C/8 * P the three
-//                                 vertical taps are ONE affine M dimension), K = 16 pixels (2 tile rows)
-// with P = HW*16, RP = (C/8)*P.  The no-swizzle descriptor mode is what makes this legal: shifting
-// the start address by one pixel (16 B) keeps every core matrix 8 x 16 B contiguous.
+// and reads it MN-major: rows = (r, ci) with row-block stride P (because RP = C/8 * P the three vertical taps are ONE
+// affine M dimension), K = 16 pixels (2 tile rows), with P = HW*16, RP = (C/8)*P.  The no-swizzle descriptor mode is
+// what makes this legal: shifting the start address by one pixel (16 B) keeps every core matrix 8 x 16 B contiguous.
 //
-// CTAs are persistent (weights stay resident across tiles); halo loads for tile i+1 (zero-filling
-// cp.async or TMA: padding by predication / out-of-bounds fill) overlap the MMAs and the epilogue of tile i.
-// One warpgroup owns the 128 x N accumulator of a tile in registers (wgmma.cuh).
+// CTAs are persistent (weights or accumulators stay resident across tiles); the halo of later tiles arrives by TMA
+// (padding = the out-of-bounds zero fill) while the MMAs and the epilogue of earlier tiles run.
+// A warpgroup owns the 128 x N accumulator of a tile in registers (wgmma.cuh).
 #include <cuda.h>
-#include <stdlib.h>
 
 #include "common.cuh"
 #include "wgmma.cuh"
@@ -127,221 +124,16 @@ template <int C, int N, int KH, int KW, int PAD>
 struct HaloCfg {
   static constexpr int CJ = C / 8;
   static constexpr int HH = TH + KH - 1, HWD = TW + KW - 1;
-  static constexpr int P = HWD * 16;            // bytes between channel chunks
-  static constexpr int RP = CJ * P;             // bytes between halo rows
-  static constexpr int HALO_BYTES = HH * RP;
   static constexpr int W_BYTES = KH * KW * C * N * 2;
-  // Halo stages per CTA.  Two stages let one CTA overlap the next tile's loads with the current MMAs, but for
-  // C = N = 64 (72 KB of resident weights) that footprint (120 KB) leaves a single 128-thread CTA per SM: latency-bound.
-  // One stage (97 KB) fits two CTAs per SM, which overlap each other instead.
-  static constexpr int NBUF = (W_BYTES + 2 * HALO_BYTES > 110 * 1024) ? 1 : 2;
 };
-
-// issue the zero-filling loads of one halo tile (all 128 threads participate)
-template <int C, int KH, int KW, int PAD, int ROWS>
-__device__ __forceinline__ void load_halo(const __nv_bfloat16* __restrict__ x, uint32_t sdst, int b, int oh0,
-                                          int ow0, int H, int W) {
-  constexpr int CJ = C / 8, HWD = TW + KW - 1;
-  constexpr int NV = ROWS * CJ * HWD;
-  for (int v = threadIdx.x; v < NV; v += 128) {
-    const int cj = v % CJ;  // channel chunk fastest: CJ consecutive threads read one pixel's C*2 contiguous bytes
-    const int t = v / CJ;
-    const int hx = t % HWD, hy = t / HWD;
-    const int ih = oh0 - PAD + hy, iw = ow0 - PAD + hx;
-    const bool ok = ih >= 0 && ih < H && iw >= 0 && iw < W;
-    const __nv_bfloat16* g = ok ? x + (((size_t)b * H + ih) * W + iw) * C + cj * 8 : x;
-    cp_async16(sdst + (uint32_t)(((hy * CJ + cj) * HWD + hx) * 16), g, ok);
-  }
-}
-
-// Register-staged variant of load_halo for the weight-gradient kernels: coalesced LDG.128 (consecutive lanes walk the
-// channel chunks of consecutive pixels of a halo row = contiguous global bytes) into registers, later STS.128 into the
-// shifted-descriptor layout (bank-conflict free per 8-lane phase).  As LDGSTS the same copies cost 2 shared-memory
-// wavefronts per lane; staged through registers they cost ~8x fewer LSU cycles, and the
-// global latency hides behind the wait for the previous tile's MMAs.
-template <int C, int KH, int KW, int PAD, int ROWS, int NTHR>
-struct HaloRegs {
-  static constexpr int CJ = C / 8, HWD = TW + KW - 1;
-  static constexpr int NV = ROWS * CJ * HWD;
-  static constexpr int PER = (NV + NTHR - 1) / NTHR;
-  uint4 v[PER];
-  __device__ __forceinline__ void load(const __nv_bfloat16* __restrict__ x, int lt, int b, int oh0, int ow0, int H, int W) {
-#pragma unroll
-    for (int i = 0; i < PER; ++i) {
-      const int idx = lt + i * NTHR;
-      uint4 r = make_uint4(0u, 0u, 0u, 0u);
-      if (idx < NV) {
-        const int cj = idx % CJ;
-        const int t = idx / CJ;
-        const int hx = t % HWD, hy = t / HWD;
-        const int ih = oh0 - PAD + hy, iw = ow0 - PAD + hx;
-        if (ih >= 0 && ih < H && iw >= 0 && iw < W)
-          r = __ldg(reinterpret_cast<const uint4*>(x + (((size_t)b * H + ih) * W + iw) * C + cj * 8));
-      }
-      v[i] = r;
-    }
-  }
-  __device__ __forceinline__ void store(uint32_t sdst, int lt) const {
-#pragma unroll
-    for (int i = 0; i < PER; ++i) {
-      const int idx = lt + i * NTHR;
-      if (idx < NV) {
-        const int cj = idx % CJ;
-        const int t = idx / CJ;
-        const int hx = t % HWD, hy = t / HWD;
-        asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(sdst + (uint32_t)(((hy * CJ + cj) * HWD + hx) * 16)),
-                     "r"(v[i].x), "r"(v[i].y), "r"(v[i].z), "r"(v[i].w) : "memory");
-      }
-    }
-  }
-};
-
-template <int C, int N, int KH, int KW, int PAD, int MODE>  // MODE 0: fwd (+stats), 1: dgrad (+addend)
-__global__ void __launch_bounds__(128) conv_halo_kernel(const HaloArgs a) {
-  using Cfg = HaloCfg<C, N, KH, KW, PAD>;
-  extern __shared__ __align__(16) uint8_t smem_raw[];
-  __shared__ float stage_buf[kStageFloats];
-  const uint32_t sbase = (smem_u32(smem_raw) + 127u) & ~127u;
-  const uint32_t s_w = sbase;
-  const uint32_t s_halo0 = s_w + Cfg::W_BYTES;
-  const int tid = threadIdx.x, lane = tid & 31;
-
-  // weights: resident for the CTA's whole life
-  {
-    const uint4* src = reinterpret_cast<const uint4*>(a.wimg);
-    for (int v = tid; v < Cfg::W_BYTES / 16; v += 128) cp_async16(s_w + (uint32_t)v * 16, src + v, true);
-  }
-  const int tiles_x = a.W / TW, tiles_y = a.H / TH;
-  const int tiles_per_img = tiles_x * tiles_y;
-  auto tile_coords = [&](int tile, int& b, int& oh0, int& ow0) {
-    b = tile / tiles_per_img;
-    const int r = tile - b * tiles_per_img;
-    oh0 = (r / tiles_x) * TH;
-    ow0 = (r % tiles_x) * TW;
-  };
-  const int first = blockIdx.x, stride = gridDim.x;
-  const int my_n = first < a.ntiles ? (a.ntiles - first + stride - 1) / stride : 0;
-  if (my_n > 0) {
-    int b, oh0, ow0;
-    tile_coords(first, b, oh0, ow0);
-    load_halo<C, KH, KW, PAD, Cfg::HH>(a.x, s_halo0, b, oh0, ow0, a.H, a.W);
-  }
-  cp_async_commit();  // group 0: weights + first halo
-  // forward: fp16 input halo x fp16 weight image; dgrad: bf16 gradients x bf16 flipped / transposed image
-  constexpr int kT = MODE == 0 ? kF16 : kBF16;
-  float acc_t[N];
-
-  const int py = tid >> 3, px = tid & 7;  // this thread's output pixel within the tile (epilogue)
-
-  constexpr int NBUF = Cfg::NBUF;
-  for (int it = 0; it < my_n; ++it) {
-    if (NBUF == 2) {
-      // prefetch the halo of tile it+1 into the stage tile it-1 used (its MMAs completed in the last iteration)
-      if (it + 1 < my_n) {
-        int b, oh0, ow0;
-        tile_coords(first + (it + 1) * stride, b, oh0, ow0);
-        load_halo<C, KH, KW, PAD, Cfg::HH>(a.x, s_halo0 + ((it + 1) & 1) * Cfg::HALO_BYTES, b, oh0, ow0, a.H, a.W);
-      }
-      cp_async_commit();
-    }
-    // halo of tile it has landed -> its MMAs
-    if (NBUF == 2) cp_async_wait<1>(); else cp_async_wait<0>();
-    fence_proxy_async_smem();
-    __syncthreads();
-    {
-      const uint32_t sh = s_halo0 + (NBUF == 2 ? (it & 1) : 0) * Cfg::HALO_BYTES;
-      wgmma_fence();
-      uint32_t accum = 0;
-#pragma unroll
-      for (int r = 0; r < KH; ++r)
-#pragma unroll
-        for (int s = 0; s < KW; ++s)
-#pragma unroll
-          for (int kk = 0; kk < C / 16; ++kk) {
-            const uint64_t da = make_smem_desc(sh + r * Cfg::RP + s * 16 + 2 * kk * Cfg::P, Cfg::P, Cfg::RP, kNoSwizzle);
-            const uint64_t db = make_smem_desc(s_w + (r * KW + s) * (C * N * 2) + 2 * kk * (N * 16), N * 16, 128, kNoSwizzle);
-            mma128<N, kT>(acc_t, da, 8 * Cfg::RP, db, accum);
-            accum = 1;
-          }
-      wgmma_commit();
-      wgmma_wait<0>();
-      acc_fence(acc_t);
-    }
-    // single halo stage: the MMAs of tile it have consumed it -> the next tile loads during this epilogue
-    if (NBUF == 1) {
-      if (it + 1 < my_n) {
-        int b, oh0, ow0;
-        tile_coords(first + (it + 1) * stride, b, oh0, ow0);
-        load_halo<C, KH, KW, PAD, Cfg::HH>(a.x, s_halo0, b, oh0, ow0, a.H, a.W);
-      }
-      cp_async_commit();
-    }
-    {   // epilogue of tile it
-      int b, oh0, ow0;
-      tile_coords(first + it * stride, b, oh0, ow0);
-      const size_t pix = ((size_t)b * a.H + oh0 + py) * a.W + ow0 + px;
-#pragma unroll
-      for (int col0 = 0; col0 < N; col0 += 32) {
-        float acc[32];
-        acc_row32(acc_t, col0, stage_buf, acc);
-        if (MODE == 0 && a.stats != nullptr) {
-          // per (frame, group) sum / sum-of-squares of this 32-column slab over the warp's 32 pixels:
-          // pairwise channel sums, then a transpose-reduce (16 + 16 shuffles instead of 2 x 16 x 5)
-          const int cpg = N / a.gn_groups;
-          float s2[16], q2[16];
-#pragma unroll
-          for (int i = 0; i < 16; ++i) {
-            s2[i] = acc[2 * i] + acc[2 * i + 1];
-            q2[i] = acc[2 * i] * acc[2 * i] + acc[2 * i + 1] * acc[2 * i + 1];
-          }
-          const float ts = warp_reduce16(s2, lane), tq = warp_reduce16(q2, lane);  // lane l: channel pair l >> 1
-          if ((lane & 1) == 0) {
-            const int ch = col0 + lane;  // first channel of the pair
-            double* dst = a.stats + ((size_t)b * a.gn_groups + ch / cpg) * 2;
-            atomicAdd(dst, (double)ts);
-            atomicAdd(dst + 1, (double)tq);
-          }
-        }
-        const size_t o = pix * N + col0;
-        if (MODE == 1 && a.addend != nullptr) {
-          const uint4* ad = reinterpret_cast<const uint4*>(a.addend + o);
-#pragma unroll
-          for (int v = 0; v < 4; ++v) {
-            float f[8];
-            unpack8(ad[v], f);
-#pragma unroll
-            for (int e = 0; e < 8; ++e) acc[v * 8 + e] += f[e];
-          }
-        }
-        uint4* dst = reinterpret_cast<uint4*>(a.y + o);
-#pragma unroll
-        for (int v = 0; v < 4; ++v) {
-          uint4 u;
-          if (MODE == 0) {  // forward output y: fp16 (saturating)
-            u.x = pack_f16x2(acc[v * 8 + 0], acc[v * 8 + 1]);
-            u.y = pack_f16x2(acc[v * 8 + 2], acc[v * 8 + 3]);
-            u.z = pack_f16x2(acc[v * 8 + 4], acc[v * 8 + 5]);
-            u.w = pack_f16x2(acc[v * 8 + 6], acc[v * 8 + 7]);
-          } else {          // data gradient: bf16
-            u.x = pack_bf16x2(acc[v * 8 + 0], acc[v * 8 + 1]);
-            u.y = pack_bf16x2(acc[v * 8 + 2], acc[v * 8 + 3]);
-            u.z = pack_bf16x2(acc[v * 8 + 4], acc[v * 8 + 5]);
-            u.w = pack_bf16x2(acc[v * 8 + 6], acc[v * 8 + 7]);
-          }
-          dst[v] = u;
-        }
-      }
-    }
-  }
-}
 
 // ------------------------------------------------------------------------------------------
 // weight gradient on the same halo buffer.  rows = (r, ci) [vertical taps form one affine M dim],
 // one accumulator per horizontal tap s and per 128-row M tile; K = output pixels.
 // ------------------------------------------------------------------------------------------
 // ring depth of conv_halo_wgrad_kernel: 4 stages where they fit beside the 17 KB accumulator transpose buffer, else 3
-constexpr int halo_wgrad_stages(int xmode, int c, int stage_bytes) {
-  return (xmode != 0 && c >= 64) ? (4 * stage_bytes <= 200 * 1024 ? 4 : 3) : 2;
+constexpr int halo_wgrad_stages(int c, int stage_bytes) {
+  return c >= 64 ? (4 * stage_bytes <= 200 * 1024 ? 4 : 3) : 2;
 }
 
 struct HaloWgradArgs {
@@ -351,12 +143,12 @@ struct HaloWgradArgs {
   int B, H, W, ntiles;
 };
 
-// XMODE: how the x halo reaches shared memory.  0 = registers / cp.async (below).  1 = one 5-D TMA box over x viewed as
+// XMODE: how the x halo reaches shared memory.  1 = one 5-D TMA box over x viewed as
 // [B, H, C/8, W, 8] (box = 8 channels x HWD pixels x C/8 chunks x halo rows = exactly the [row][chunk][pixel] layout the
 // shifted descriptors read).  2 = the same over the 2x2 SPACE-TO-DEPTH view of a tensor with C/4 real channels: a
 // 3x3 stride-2 pad-1 conv of x is a 2x2 stride-1 pad-1 conv of the view (csrc/conv_s2.cu), whose block row `by` is image
 // rows 2by, 2by+1 -- the box simply covers twice the rows of the real tensor with (dx, c) as the chunk dimension.
-template <int C, int N, int KH, int KW, int PAD, int XMODE = 0>
+template <int C, int N, int KH, int KW, int PAD, int XMODE>
 __global__ void __launch_bounds__(128)
 conv_halo_wgrad_kernel(const HaloWgradArgs a, const __grid_constant__ CUtensorMap tmap_dy,
                        const __grid_constant__ CUtensorMap tmap_x) {
@@ -372,7 +164,7 @@ conv_halo_wgrad_kernel(const HaloWgradArgs a, const __grid_constant__ CUtensorMa
   // Ring depth.  With the x halo AND the dy tile arriving by TMA, two stages expose the load latency of a tile once per
   // tile (its MMAs are much shorter): the wide configurations, one CTA per SM anyway (shared memory), prefetch NSW-1 tiles
   // ahead; the 32-channel layers and the stem keep two stages and more CTAs per SM instead.
-  constexpr int NSW = halo_wgrad_stages(XMODE, C, STAGE);
+  constexpr int NSW = halo_wgrad_stages(C, STAGE);
   // accumulators (s, mt) of 128 rows x N: a CTA holds APC of them in registers (<= 128 columns), blockIdx.y picks the group
   constexpr int NACC = KW * MT;
   constexpr int APC = NACC * N <= 128 ? NACC : 128 / N;
@@ -405,30 +197,15 @@ conv_halo_wgrad_kernel(const HaloWgradArgs a, const __grid_constant__ CUtensorMa
     oh0 = (r / tiles_x) * TH;
     ow0 = (r % tiles_x) * TW;
   };
-  // x halo: zero-filling cp.async into the shifted-descriptor layout (all threads).  dy tile: ONE TMA box (N channels x
-  // 8 x 16 pixels) into the MN-major swizzled layout -- as LDGSTS it was a transpose (pixel-major tensor -> channel-chunk-
-  // major rows), 2 shared-memory wavefronts per 16-byte copy, which made this kernel LSU-bound (see the small-image
-  // kernel below).
-  // Register staging pays while the halo is <= 8 vectors per thread (C <= 32, the stem); for C = 64 (12 vectors, 128
-  // registers) the lost occupancy costs more than the LDGSTS wavefronts: cp.async there.
-  constexpr bool kRegStage = XMODE == 0 && HROWS_LOAD * CJ * HWD <= 128 * 8;
-  HaloRegs<C, KH, KW, PAD, kRegStage ? HROWS_LOAD : 1, 128> xr;   // the x halo of the NEXT tile, in flight in registers
-  auto fetch_x = [&](int tile) {
-    if (!kRegStage) return;
-    int b, oh0, ow0;
-    tile_coords(tile, b, oh0, ow0);
-    xr.load(reinterpret_cast<const __nv_bfloat16*>(a.x), tid, b, oh0, ow0, a.H, a.W);
-  };
-  auto commit_tile = [&, tmap_p, tmap_xp](int tile, int st) {   // stage `st` is free: x halo -> smem, dy tile by TMA
+  // dy tile: ONE TMA box (N channels x 8 x 16 pixels) into the MN-major swizzled layout -- as LDGSTS it was a transpose
+  // (pixel-major tensor -> channel-chunk-major rows), 2 shared-memory wavefronts per 16-byte copy, which made this kernel
+  // LSU-bound (see the small-image kernel below).
+  auto commit_tile = [&, tmap_p, tmap_xp](int tile, int st) {   // stage `st` is free: x halo and dy tile by TMA
     int b, oh0, ow0;
     tile_coords(tile, b, oh0, ow0);
     const uint32_t sd = sbase + st * STAGE;
-    if (XMODE == 0) {
-      if (kRegStage) xr.store(sd + DY_BYTES, tid);
-      else load_halo<C, KH, KW, PAD, HROWS_LOAD>(a.x, sd + DY_BYTES, b, oh0, ow0, a.H, a.W);
-    }
     if (tid == 0) {
-      mbar_expect_tx(&dy_bar[st], (uint32_t)(DY_BYTES + (XMODE ? HROWS_LOAD * RP : 0)));
+      mbar_expect_tx(&dy_bar[st], (uint32_t)(DY_BYTES + HROWS_LOAD * RP));
       tma_load_4d(sd, tmap_p, &dy_bar[st], 0, ow0, oh0, b);
       // coordinates (channel-in-chunk, pixel column, chunk, row, frame); space-to-depth: rows of the REAL tensor
       if (XMODE == 1) tma_load_5d(sd + DY_BYTES, tmap_xp, &dy_bar[st], 0, ow0 - PAD, 0, oh0 - PAD, b);
@@ -437,10 +214,6 @@ conv_halo_wgrad_kernel(const HaloWgradArgs a, const __grid_constant__ CUtensorMa
   };
   const int first = blockIdx.x, stride = gridDim.x;
   const int my_n = first < a.ntiles ? (a.ntiles - first + stride - 1) / stride : 0;
-  if (XMODE == 0 && my_n > 0) {
-    fetch_x(first);
-    commit_tile(first, 0);
-  }
   cp_async_commit();
   fence_proxy_async_smem();
   __syncthreads();
@@ -465,28 +238,14 @@ conv_halo_wgrad_kernel(const HaloWgradArgs a, const __grid_constant__ CUtensorMa
     wgmma_wait<0>();
   };
 
-  if (XMODE != 0) {
-    // both operands by TMA: thread 0 keeps NSW-1 tiles of loads ahead of the tensor core
-    if (tid == 0)
-      for (int p = 0; p < NSW - 1 && p < my_n; ++p) commit_tile(first + p * stride, p);
-    for (int it = 0; it < my_n; ++it) {
-      const int nxt = it + NSW - 1;   // its stage was read by the MMAs of tile it-1, complete
-      if (tid == 0 && nxt < my_n) commit_tile(first + nxt * stride, nxt % NSW);
-      mbar_wait(&dy_bar[it % NSW], (it / NSW) & 1);
-      mma_tile(it, sbase + (it % NSW) * STAGE);
-    }
-  } else {
-    for (int it = 0; it < my_n; ++it) {
-      const bool more = it + 1 < my_n;
-      if (more) fetch_x(first + (it + 1) * stride);                 // global loads in flight ...
-      if (more) commit_tile(first + (it + 1) * stride, (it + 1) & 1);   // ... into the stage tile it-1 used
-      cp_async_commit();
-      cp_async_wait<1>();         // cp.async variant: this thread's copies of tile it (issued an iteration ago)
-      fence_proxy_async_smem();   // st.shared / cp.async (generic proxy) -> wgmma (async proxy)
-      __syncthreads();
-      mbar_wait(&dy_bar[it & 1], (it >> 1) & 1);   // the TMA'd dy tile
-      mma_tile(it, sbase + (it & 1) * STAGE);
-    }
+  // both operands by TMA: thread 0 keeps NSW-1 tiles of loads ahead of the tensor core
+  if (tid == 0)
+    for (int p = 0; p < NSW - 1 && p < my_n; ++p) commit_tile(first + p * stride, p);
+  for (int it = 0; it < my_n; ++it) {
+    const int nxt = it + NSW - 1;   // its stage was read by the MMAs of tile it-1, complete
+    if (tid == 0 && nxt < my_n) commit_tile(first + nxt * stride, nxt % NSW);
+    mbar_wait(&dy_bar[it % NSW], (it / NSW) & 1);
+    mma_tile(it, sbase + (it % NSW) * STAGE);
   }
   {   // a worker without tiles still writes its (zero) partial
 #pragma unroll
@@ -702,297 +461,26 @@ __global__ void unpack_stem_wgrad_kernel(const float* __restrict__ acc, float* _
   }
 }
 
-// resident CTAs per SM from static limits (registers, shared memory); cached per kernel
-// ------------------------------------------------------------------------------------------
-// The same persistent forward / dgrad kernel with the halo loaded by TMA (HB200_NO_HALO_TMA=1 falls back to the cp.async
-// kernel above).  One thread issues C/8
-// `cp.async.bulk.tensor.4d` box copies per tile (box = {8 channels, halo width, halo height, 1 frame}; the conv
-// padding is the TMA unit's out-of-bounds zero fill) that complete on an mbarrier, instead of ~6 predicated
-// cp.async per thread -- the address / predicate arithmetic that makes conv_halo_kernel<32,32> issue-bound.
-// The box lands as [cj][hy][hx][8 ch], so the K-major descriptors become
-//   start = stage + 2kk*SLAB + r*HWD*16 + s*16,   LBO = SLAB (next 8 channels),   SBO = HWD*16 (next tile row).
-// The warpgroup waits for the load on the stage's mbarrier before it issues the tile's MMAs.
-// ------------------------------------------------------------------------------------------
-
-template <int C, int N, int KH, int KW, int PAD, int MODE>
-__global__ void __launch_bounds__(128)
-conv_halo_tma_kernel(const HaloArgs a, const __grid_constant__ CUtensorMap tmap) {
-  using Cfg = HaloCfg<C, N, KH, KW, PAD>;
-  constexpr int CJ = Cfg::CJ, HH = Cfg::HH, HWD = Cfg::HWD;
-  constexpr uint32_t SLAB = (uint32_t)((HH * HWD * 16 + 127) / 128 * 128);
-  constexpr uint32_t STAGE = CJ * SLAB;
-  // halo stages: two when they fit next to the resident weights with >= 2 CTAs per SM; ONE for C = N = 64 (72 KB of
-  // weights): the load of tile it+1 then starts when the MMAs of tile it are done, and the second CTA on the SM covers
-  // the gap -- like conv_halo_kernel, minus the 2880 LSU cycles per tile its cp.async halo gather costs
-  constexpr int NB = (Cfg::W_BYTES + 2 * (int)STAGE > 110 * 1024) ? 1 : 2;
-  extern __shared__ __align__(16) uint8_t smem_raw[];
-  __shared__ __align__(8) uint64_t ld_bar[2];
-  __shared__ float stage_buf[kStageFloats];
-  const uint32_t sbase = (smem_u32(smem_raw) + 127u) & ~127u;
-  const uint32_t s_w = sbase;
-  const uint32_t s_halo0 = s_w + Cfg::W_BYTES;   // W_BYTES is a multiple of 128
-  const int tid = threadIdx.x, lane = tid & 31;
-
-  if (tid == 0) {
-    mbar_init(&ld_bar[0], 1);
-    mbar_init(&ld_bar[1], 1);
-    mbar_fence_init();
-  }
-  {
-    const uint4* src = reinterpret_cast<const uint4*>(a.wimg);
-    for (int v = tid; v < Cfg::W_BYTES / 16; v += 128) cp_async16(s_w + (uint32_t)v * 16, src + v, true);
-  }
-  cp_async_commit();
-  const int tiles_x = a.W / TW, tiles_y = a.H / TH;
-  const int tiles_per_img = tiles_x * tiles_y;
-  auto tile_coords = [&](int tile, int& b, int& oh0, int& ow0) {
-    b = tile / tiles_per_img;
-    const int r = tile - b * tiles_per_img;
-    oh0 = (r / tiles_x) * TH;
-    ow0 = (r % tiles_x) * TW;
-  };
-  // The descriptor must be addressed in PARAM space: `&tmap` evaluated here, in the kernel body.  Inside the lambda a
-  // by-reference capture makes nvcc spill a thread-local copy of the 128-byte map and hand the TMA unit a stack
-  // address (round-1 version: every tile loaded garbage).
-  const CUtensorMap* const tmap_p = &tmap;
-  auto issue_halo = [&, tmap_p](int tile, int stage) {   // thread 0 only
-    int b, oh0, ow0;
-    tile_coords(tile, b, oh0, ow0);
-    mbar_expect_tx(&ld_bar[stage], (uint32_t)(CJ * HH * HWD * 16));
-#pragma unroll
-    for (int j = 0; j < CJ; ++j)
-      tma_load_4d(s_halo0 + (uint32_t)stage * STAGE + (uint32_t)j * SLAB, tmap_p, &ld_bar[stage], j * 8, ow0 - PAD,
-                  oh0 - PAD, b);
-  };
-  const int first = blockIdx.x, stride = gridDim.x;
-  const int my_n = first < a.ntiles ? (a.ntiles - first + stride - 1) / stride : 0;
-  __syncthreads();   // barriers initialised
-  if (tid == 0 && my_n > 0) issue_halo(first, 0);
-  cp_async_wait<0>();          // weights
-  fence_proxy_async_smem();    // cp.async (generic proxy) -> wgmma (async proxy)
-  __syncthreads();
-  // forward: fp16 input halo x fp16 weight image; dgrad: bf16 gradients x bf16 flipped / transposed image
-  constexpr int kT = MODE == 0 ? kF16 : kBF16;
-  float acc_t[N];
-  const int py = tid >> 3, px = tid & 7;
-
-  for (int it = 0; it < my_n; ++it) {
-    // two stages: tile it+1 loads into the stage tile it-1 used (its MMAs completed in the last iteration)
-    if (NB == 2 && tid == 0 && it + 1 < my_n) issue_halo(first + (it + 1) * stride, (it + 1) & 1);
-    mbar_wait(&ld_bar[NB == 2 ? (it & 1) : 0], NB == 2 ? ((it >> 1) & 1) : (it & 1));
-    {
-      const uint32_t sh = s_halo0 + (uint32_t)(NB == 2 ? (it & 1) : 0) * STAGE;
-      wgmma_fence();
-      uint32_t accum = 0;
-#pragma unroll
-      for (int r = 0; r < KH; ++r)
-#pragma unroll
-        for (int s = 0; s < KW; ++s)
-#pragma unroll
-          for (int kk = 0; kk < C / 16; ++kk) {
-            const uint64_t da = make_smem_desc(sh + 2 * kk * SLAB + r * (HWD * 16) + s * 16, SLAB, HWD * 16, kNoSwizzle);
-            const uint64_t db = make_smem_desc(s_w + (r * KW + s) * (C * N * 2) + 2 * kk * (N * 16), N * 16, 128, kNoSwizzle);
-            mma128<N, kT>(acc_t, da, 8 * HWD * 16, db, accum);
-            accum = 1;
-          }
-      wgmma_commit();
-      wgmma_wait<0>();
-      acc_fence(acc_t);
-    }
-    // single halo stage: the MMAs of tile it have consumed it -> the next tile loads during this epilogue
-    if (NB == 1 && tid == 0 && it + 1 < my_n) issue_halo(first + (it + 1) * stride, 0);
-    {   // epilogue of tile it
-      int b, oh0, ow0;
-      tile_coords(first + it * stride, b, oh0, ow0);
-      const size_t pix = ((size_t)b * a.H + oh0 + py) * a.W + ow0 + px;
-#pragma unroll
-      for (int col0 = 0; col0 < N; col0 += 32) {
-        float acc[32];
-        acc_row32(acc_t, col0, stage_buf, acc);
-        if (MODE == 0 && a.stats != nullptr)
-          halo_gn_stats_chunk(acc, lane, N / a.gn_groups, a.stats + (size_t)b * a.gn_groups * 2, col0);
-        const size_t o = pix * N + col0;
-        if (MODE == 1 && a.addend != nullptr) {
-          const uint4* ad = reinterpret_cast<const uint4*>(a.addend + o);
-#pragma unroll
-          for (int v = 0; v < 4; ++v) {
-            float f[8];
-            unpack8(ad[v], f);
-#pragma unroll
-            for (int e = 0; e < 8; ++e) acc[v * 8 + e] += f[e];
-          }
-        }
-        uint4* dst = reinterpret_cast<uint4*>(a.y + o);
-#pragma unroll
-        for (int v = 0; v < 4; ++v) {
-          uint4 u;
-          if (MODE == 0) {  // forward output y: fp16 (saturating)
-            u.x = pack_f16x2(acc[v * 8 + 0], acc[v * 8 + 1]);
-            u.y = pack_f16x2(acc[v * 8 + 2], acc[v * 8 + 3]);
-            u.z = pack_f16x2(acc[v * 8 + 4], acc[v * 8 + 5]);
-            u.w = pack_f16x2(acc[v * 8 + 6], acc[v * 8 + 7]);
-          } else {          // data gradient: bf16
-            u.x = pack_bf16x2(acc[v * 8 + 0], acc[v * 8 + 1]);
-            u.y = pack_bf16x2(acc[v * 8 + 2], acc[v * 8 + 3]);
-            u.z = pack_bf16x2(acc[v * 8 + 4], acc[v * 8 + 5]);
-            u.w = pack_bf16x2(acc[v * 8 + 6], acc[v * 8 + 7]);
-          }
-          dst[v] = u;
-        }
-      }
-    }
-  }
-}
-
-template <int C, int N, int MODE>
-__global__ void __launch_bounds__(128)
-conv_halo_sw_kernel(const HaloArgs a, const __grid_constant__ CUtensorMap tmap) {
-  // 3x3 stride-1 pad-1.  The halo is staged as KW = 3 copies of the tile rows, copy kx pre-shifted by kx pixels, each
-  // copy [HH rows][8 pixels][C channels] in the 64- / 128-byte-swizzle K-major layout (one TMA box per copy: rows of
-  // C*2 bytes instead of the 16-byte pieces of the no-swizzle slabs, whose rate -- not bytes -- bounds the slab-fed
-  // kernels).  A filter tap (r, s) is then copy s shifted by r whole swizzle atoms: aligned descriptors only.
-  using Cfg = HaloCfg<C, N, 3, 3, 1>;
-  constexpr int KH = 3, KW = 3, PAD = 1, HH = Cfg::HH;
-  constexpr uint32_t RB = C * 2;                 // bytes per pixel row of the operand: 64 (SWIZZLE_64B) or 128
-  constexpr uint32_t ATOM = 8 * RB;              // 8 pixels = one output row of the tile = one swizzle atom
-  constexpr uint32_t COPY = HH * ATOM;
-  constexpr uint32_t STAGE = KW * COPY;
-  constexpr int NB = (Cfg::W_BYTES + 2 * (int)STAGE > 200 * 1024) ? 1 : 2;
-  constexpr int kSw = RB == 128 ? kSwizzle128B : kSwizzle64B;
-  static_assert(RB == 64 || RB == 128, "conv_halo_sw: 32 or 64 channels");
-  extern __shared__ __align__(16) uint8_t smem_raw[];
-  __shared__ __align__(8) uint64_t ld_bar[2];
-  __shared__ float stage_buf[kStageFloats];
-  const uint32_t sbase = (smem_u32(smem_raw) + 1023u) & ~1023u;   // swizzle atoms: 1024-byte aligned
-  const uint32_t s_w = sbase;
-  const uint32_t s_halo0 = s_w + Cfg::W_BYTES;   // W_BYTES is a multiple of 128
-  const int tid = threadIdx.x, lane = tid & 31;
-
-  if (tid == 0) {
-    mbar_init(&ld_bar[0], 1);
-    mbar_init(&ld_bar[1], 1);
-    mbar_fence_init();
-  }
-  {
-    const uint4* src = reinterpret_cast<const uint4*>(a.wimg);
-    for (int v = tid; v < Cfg::W_BYTES / 16; v += 128) cp_async16(s_w + (uint32_t)v * 16, src + v, true);
-  }
-  cp_async_commit();
-  const int tiles_x = a.W / TW, tiles_y = a.H / TH;
-  const int tiles_per_img = tiles_x * tiles_y;
-  auto tile_coords = [&](int tile, int& b, int& oh0, int& ow0) {
-    b = tile / tiles_per_img;
-    const int r = tile - b * tiles_per_img;
-    oh0 = (r / tiles_x) * TH;
-    ow0 = (r % tiles_x) * TW;
-  };
-  // The descriptor must be addressed in PARAM space: `&tmap` evaluated here, in the kernel body.  Inside the lambda a
-  // by-reference capture makes nvcc spill a thread-local copy of the 128-byte map and hand the TMA unit a stack
-  // address (round-1 version: every tile loaded garbage).
-  const CUtensorMap* const tmap_p = &tmap;
-  auto issue_halo = [&, tmap_p](int tile, int stage) {   // thread 0 only
-    int b, oh0, ow0;
-    tile_coords(tile, b, oh0, ow0);
-    mbar_expect_tx(&ld_bar[stage], STAGE);
-#pragma unroll
-    for (int kx = 0; kx < KW; ++kx)
-      tma_load_4d(s_halo0 + (uint32_t)stage * STAGE + (uint32_t)kx * COPY, tmap_p, &ld_bar[stage], 0, ow0 - PAD + kx,
-                  oh0 - PAD, b);
-  };
-  const int first = blockIdx.x, stride = gridDim.x;
-  const int my_n = first < a.ntiles ? (a.ntiles - first + stride - 1) / stride : 0;
-  __syncthreads();   // barriers initialised
-  if (tid == 0 && my_n > 0) issue_halo(first, 0);
-  cp_async_wait<0>();          // weights
-  fence_proxy_async_smem();    // cp.async (generic proxy) -> wgmma (async proxy)
-  __syncthreads();
-  // forward: fp16 input halo x fp16 weight image; dgrad: bf16 gradients x bf16 flipped / transposed image
-  constexpr int kT = MODE == 0 ? kF16 : kBF16;
-  float acc_t[N];
-  const int py = tid >> 3, px = tid & 7;
-
-  for (int it = 0; it < my_n; ++it) {
-    // two stages: tile it+1 loads into the stage tile it-1 used (its MMAs completed in the last iteration)
-    if (NB == 2 && tid == 0 && it + 1 < my_n) issue_halo(first + (it + 1) * stride, (it + 1) & 1);
-    mbar_wait(&ld_bar[NB == 2 ? (it & 1) : 0], NB == 2 ? ((it >> 1) & 1) : (it & 1));
-    {
-      const uint32_t sh = s_halo0 + (uint32_t)(NB == 2 ? (it & 1) : 0) * STAGE;
-      wgmma_fence();
-      uint32_t accum = 0;
-#pragma unroll
-      for (int r = 0; r < KH; ++r)
-#pragma unroll
-        for (int s = 0; s < KW; ++s)
-#pragma unroll
-          for (int kk = 0; kk < C / 16; ++kk) {
-            const uint64_t da = make_smem_desc(sh + s * COPY + r * ATOM + kk * 32, 16, ATOM, (Layout)kSw);
-            const uint64_t db = make_smem_desc(s_w + (r * KW + s) * (C * N * 2) + 2 * kk * (N * 16), N * 16, 128, kNoSwizzle);
-            mma128<N, kT>(acc_t, da, 8 * ATOM, db, accum);
-            accum = 1;
-          }
-      wgmma_commit();
-      wgmma_wait<0>();
-      acc_fence(acc_t);
-    }
-    // single halo stage: the MMAs of tile it have consumed it -> the next tile loads during this epilogue
-    if (NB == 1 && tid == 0 && it + 1 < my_n) issue_halo(first + (it + 1) * stride, 0);
-    {   // epilogue of tile it
-      int b, oh0, ow0;
-      tile_coords(first + it * stride, b, oh0, ow0);
-      const size_t pix = ((size_t)b * a.H + oh0 + py) * a.W + ow0 + px;
-#pragma unroll
-      for (int col0 = 0; col0 < N; col0 += 32) {
-        float acc[32];
-        acc_row32(acc_t, col0, stage_buf, acc);
-        if (MODE == 0 && a.stats != nullptr)
-          halo_gn_stats_chunk(acc, lane, N / a.gn_groups, a.stats + (size_t)b * a.gn_groups * 2, col0);
-        const size_t o = pix * N + col0;
-        if (MODE == 1 && a.addend != nullptr) {
-          const uint4* ad = reinterpret_cast<const uint4*>(a.addend + o);
-#pragma unroll
-          for (int v = 0; v < 4; ++v) {
-            float f[8];
-            unpack8(ad[v], f);
-#pragma unroll
-            for (int e = 0; e < 8; ++e) acc[v * 8 + e] += f[e];
-          }
-        }
-        uint4* dst = reinterpret_cast<uint4*>(a.y + o);
-#pragma unroll
-        for (int v = 0; v < 4; ++v) {
-          uint4 u;
-          if (MODE == 0) {  // forward output y: fp16 (saturating)
-            u.x = pack_f16x2(acc[v * 8 + 0], acc[v * 8 + 1]);
-            u.y = pack_f16x2(acc[v * 8 + 2], acc[v * 8 + 3]);
-            u.z = pack_f16x2(acc[v * 8 + 4], acc[v * 8 + 5]);
-            u.w = pack_f16x2(acc[v * 8 + 6], acc[v * 8 + 7]);
-          } else {          // data gradient: bf16
-            u.x = pack_bf16x2(acc[v * 8 + 0], acc[v * 8 + 1]);
-            u.y = pack_bf16x2(acc[v * 8 + 2], acc[v * 8 + 3]);
-            u.z = pack_bf16x2(acc[v * 8 + 4], acc[v * 8 + 5]);
-            u.w = pack_bf16x2(acc[v * 8 + 6], acc[v * 8 + 7]);
-          }
-          dst[v] = u;
-        }
-      }
-    }
-  }
-}
-
-
-// ---- warp-specialised variant ---------------------------------------------------------------------------------------
-// conv_halo_tma_kernel runs load -> MMA -> epilogue of consecutive tiles from one program order: with a single halo
-// stage the TMA latency of tile it+1 is exposed after every tile, and only a second CTA of the SM hides it.  Here the
-// loads run in their own warp and meet the consumers only at mbarriers:
-//   warp 8 (one lane)  producer: halo stage ring, NS deep (as many as fit next to the resident weights)
+// ---- forward / dgrad: persistent, warp-specialised, halo by TMA ------------------------------------------------------
+// One thread issues the halo's TMA box copies per tile (the conv padding is the TMA unit's out-of-bounds zero fill),
+// which complete on an mbarrier.  A zero-filling cp.async gather needs ~6 predicated copies per thread per tile, and
+// that address / predicate arithmetic made the 32-channel kernel issue-bound.  The halo lands in one of two layouts:
+//   slabs (SW = false, the stem): C/8 boxes of {8 channels, halo width, halo height}, i.e. [cj][hy][hx][8 ch]; tap (r, s)
+//        reads  start = stage + 2kk*SLAB + r*HWD*16 + s*16,  LBO = SLAB (next 8 channels),  SBO = HWD*16 (next tile row)
+//   swizzled rows (SW = true, the 32- / 64-channel layers): KW copies of the tile rows, copy kx pre-shifted by kx
+//        pixels, each [HH rows][8 pixels][C channels] in the 64- / 128-byte-swizzle K-major layout, one box per copy.
+//        Its rows of C*2 bytes replace the 16-byte pieces of the slabs, whose rate -- not bytes -- bounds a slab-fed
+//        kernel; tap (r, s) is copy s shifted by r whole swizzle atoms: aligned descriptors only, at KW times the bytes.
+// With load -> MMA -> epilogue of consecutive tiles in one program order, the TMA latency of tile it+1 is exposed after
+// every tile, and only a second CTA of the SM hides it.  Here the loads run in their own warp and meet the consumers
+// only at mbarriers:
+//   warp 8 (one lane)  producer: halo stage ring, NS deep
 //   warps 0-3, 4-7     two consumer warpgroups; tile `it` of the CTA goes to warpgroup it & 1.  Each waits full[stage],
 //                      issues the tile's MMAs, releases the stage (empty[stage]) as soon as they complete, then runs the
 //                      GroupNorm sums / addend / pack / store while the other warpgroup's MMAs run on the next tile
 // The accumulator lives in registers, so one warpgroup cannot overlap its own epilogue with MMAs: the second one is what
 // keeps the tensor core busy.  Each warpgroup transposes through its own stage buffer (dynamic shared memory, after the
 // halo ring) under its own named barrier (1 + warpgroup).
-// SW: stage the halo as KW pre-shifted copies of whole pixel rows in the swizzled K-major layout (conv_halo_sw_kernel)
-// instead of 16-byte channel slabs: aligned operand reads for the MMAs at KW times the TMA bytes
 constexpr int kHaloWsThreads = 288;
 template <int C, int N, int KH, int KW, int PAD, int MODE, int NS, bool SW = false>
 __global__ void __launch_bounds__(kHaloWsThreads)
@@ -1154,57 +642,6 @@ static int blocks_per_sm(const void* kern, size_t smem, int* cache, int threads 
   return n;
 }
 
-template <int C, int N, int KH, int KW, int PAD, int MODE>
-static int launch_halo(const HaloArgs& a, cudaStream_t st) {
-  using Cfg = HaloCfg<C, N, KH, KW, PAD>;
-  const size_t smem = Cfg::W_BYTES + Cfg::NBUF * Cfg::HALO_BYTES + 256;
-  auto kern = conv_halo_kernel<C, N, KH, KW, PAD, MODE>;
-  static int cache = 0;
-  if (cache == 0) HB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  const int per_sm = blocks_per_sm((const void*)kern, smem, &cache);
-  int grid = kNumSMs * per_sm;
-  if (grid > a.ntiles) grid = a.ntiles;
-  kern<<<grid, 128, smem, st>>>(a);
-  HB_LAUNCH_OK();
-  count_launch(1);
-  return HB200_OK;
-}
-
-template <int C, int N, int KH, int KW, int PAD, int MODE>
-static int launch_halo_tma(const HaloArgs& a, cudaStream_t st) {
-  using Cfg = HaloCfg<C, N, KH, KW, PAD>;
-  EncodeTiledFn enc = halo_encode_fn();
-  if (!enc) {
-    set_last_error("conv_halo (TMA): cuTensorMapEncodeTiled is not available from this driver");
-    return HB200_ERR_UNSUPPORTED;
-  }
-  CUtensorMap tmap;
-  const cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)a.W, (cuuint64_t)a.H, (cuuint64_t)a.B};
-  const cuuint64_t strides[3] = {(cuuint64_t)C * 2, (cuuint64_t)a.W * C * 2, (cuuint64_t)a.H * a.W * C * 2};
-  const cuuint32_t box[4] = {8u, (cuuint32_t)Cfg::HWD, (cuuint32_t)Cfg::HH, 1u};
-  const cuuint32_t estr[4] = {1u, 1u, 1u, 1u};
-  const CUresult r = enc(&tmap, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, (void*)a.x, dims, strides, box, estr,
-                         CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) {
-    set_last_error("conv_halo (TMA): cuTensorMapEncodeTiled failed (%d)", (int)r);
-    return HB200_ERR_CUDA;
-  }
-  constexpr size_t slab = (size_t)((Cfg::HH * Cfg::HWD * 16 + 127) / 128 * 128);
-  constexpr int nstage = (Cfg::W_BYTES + 2 * (int)(Cfg::CJ * slab) > 110 * 1024) ? 1 : 2;
-  const size_t smem = Cfg::W_BYTES + nstage * Cfg::CJ * slab + 256;
-  auto kern = conv_halo_tma_kernel<C, N, KH, KW, PAD, MODE>;
-  static int cache = 0;
-  if (cache == 0) HB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  const int per_sm = blocks_per_sm((const void*)kern, smem, &cache);
-  int grid = kNumSMs * per_sm;
-  if (grid > a.ntiles) grid = a.ntiles;
-  kern<<<grid, 128, smem, st>>>(a, tmap);
-  HB_LAUNCH_OK();
-  count_launch(1);
-  return HB200_OK;
-}
-
 template <int C, int N, int KH, int KW, int PAD, int MODE, int NS, bool SW = false>
 static int launch_halo_ws(const HaloArgs& a, cudaStream_t st) {
   using Cfg = HaloCfg<C, N, KH, KW, PAD>;
@@ -1253,47 +690,12 @@ static int launch_halo_ws(const HaloArgs& a, cudaStream_t st) {
   return HB200_OK;
 }
 
-template <int C, int N, int MODE>
-static int launch_halo_sw(const HaloArgs& a, cudaStream_t st) {
-  using Cfg = HaloCfg<C, N, 3, 3, 1>;
-  EncodeTiledFn enc = halo_encode_fn();
-  if (!enc) {
-    set_last_error("conv_halo (swizzled TMA): cuTensorMapEncodeTiled is not available from this driver");
-    return HB200_ERR_UNSUPPORTED;
-  }
-  CUtensorMap tmap;
-  const cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)a.W, (cuuint64_t)a.H, (cuuint64_t)a.B};
-  const cuuint64_t strides[3] = {(cuuint64_t)C * 2, (cuuint64_t)a.W * C * 2, (cuuint64_t)a.H * a.W * C * 2};
-  const cuuint32_t box[4] = {(cuuint32_t)C, (cuuint32_t)TW, (cuuint32_t)Cfg::HH, 1u};   // whole pixels: C*2-byte rows
-  const cuuint32_t estr[4] = {1u, 1u, 1u, 1u};
-  const CUresult r = enc(&tmap, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, (void*)a.x, dims, strides, box, estr,
-                         CU_TENSOR_MAP_INTERLEAVE_NONE, C == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B,
-                         CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) {
-    set_last_error("conv_halo (swizzled TMA): cuTensorMapEncodeTiled failed (%d)", (int)r);
-    return HB200_ERR_CUDA;
-  }
-  constexpr size_t stage = (size_t)3 * Cfg::HH * 8 * C * 2;
-  constexpr int nstage = (Cfg::W_BYTES + 2 * (int)stage > 200 * 1024) ? 1 : 2;
-  const size_t smem = Cfg::W_BYTES + nstage * stage + 1024;
-  auto kern = conv_halo_sw_kernel<C, N, MODE>;
-  static int cache = 0;
-  if (cache == 0) HB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  const int per_sm = blocks_per_sm((const void*)kern, smem, &cache);
-  int grid = kNumSMs * per_sm;
-  if (grid > a.ntiles) grid = a.ntiles;
-  kern<<<grid, 128, smem, st>>>(a, tmap);
-  HB_LAUNCH_OK();
-  count_launch(1);
-  return HB200_OK;
-}
-
-template <int C, int N, int KH, int KW, int PAD, int XMODE = 0>
+template <int C, int N, int KH, int KW, int PAD, int XMODE>
 static int launch_halo_wgrad(const HaloWgradArgs& a, cudaStream_t st) {
   constexpr int CJ = C / 8, HWD = TW + KW - 1, P = HWD * 16, RP = CJ * P;
   constexpr int MT = (KH * CJ + 15) / 16, RMAX = (MT * 16 + CJ - 1) / CJ, HROWS = TH - 1 + RMAX;
   constexpr int STAGE = (128 * N * 2 + HROWS * RP + 1023) / 1024 * 1024;
-  constexpr int NSW = halo_wgrad_stages(XMODE, C, STAGE);
+  constexpr int NSW = halo_wgrad_stages(C, STAGE);
   const size_t smem = NSW * (size_t)STAGE + 1024 + 64;
   EncodeTiledFn enc = halo_encode_fn();
   if (!enc) {
@@ -1316,23 +718,21 @@ static int launch_halo_wgrad(const HaloWgradArgs& a, cudaStream_t st) {
   // x halo by TMA: x bf16 [B, Hx, Wx, Cx] seen as (8 | pixel column | chunk | row | frame).  XMODE 2: a.H, a.W are the
   // dims of the space-to-depth view; the real tensor has 2H x 2W pixels of C/4 channels, "pixel column" steps over
   // pixel PAIRS (2 * Cx * 2 bytes) and a row of the view's chunks = the (dx, c) run of one image row
-  CUtensorMap tmap_x = tmap;
-  if (XMODE != 0) {
-    const int cx = XMODE == 2 ? C / 4 : C, hx = XMODE == 2 ? 2 * a.H : a.H, wx = XMODE == 2 ? 2 * a.W : a.W;
-    const int chunks_per_row = XMODE == 2 ? CJ / 2 : CJ, col_bytes = (XMODE == 2 ? 2 : 1) * cx * 2;
-    const cuuint64_t xd[5] = {8u, (cuuint64_t)a.W, (cuuint64_t)chunks_per_row, (cuuint64_t)hx, (cuuint64_t)a.B};
-    const cuuint64_t xs[4] = {(cuuint64_t)col_bytes, 16u, (cuuint64_t)wx * cx * 2, (cuuint64_t)hx * wx * cx * 2};
-    constexpr int HROWS_LOAD = TH + KH - 1;
-    const cuuint32_t xb[5] = {8u, (cuuint32_t)HWD, (cuuint32_t)chunks_per_row,
-                              (cuuint32_t)(XMODE == 2 ? 2 * HROWS_LOAD : HROWS_LOAD), 1u};
-    const cuuint32_t xe[5] = {1u, 1u, 1u, 1u, 1u};
-    const CUresult rx = enc(&tmap_x, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 5, (void*)a.x, xd, xs, xb, xe,
-                            CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                            CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (rx != CUDA_SUCCESS) {
-      set_last_error("conv_halo_wgrad: cuTensorMapEncodeTiled (x halo) failed (%d)", (int)rx);
-      return HB200_ERR_CUDA;
-    }
+  CUtensorMap tmap_x;
+  const int cx = XMODE == 2 ? C / 4 : C, hx = XMODE == 2 ? 2 * a.H : a.H, wx = XMODE == 2 ? 2 * a.W : a.W;
+  const int chunks_per_row = XMODE == 2 ? CJ / 2 : CJ, col_bytes = (XMODE == 2 ? 2 : 1) * cx * 2;
+  const cuuint64_t xd[5] = {8u, (cuuint64_t)a.W, (cuuint64_t)chunks_per_row, (cuuint64_t)hx, (cuuint64_t)a.B};
+  const cuuint64_t xs[4] = {(cuuint64_t)col_bytes, 16u, (cuuint64_t)wx * cx * 2, (cuuint64_t)hx * wx * cx * 2};
+  constexpr int HROWS_LOAD = TH + KH - 1;
+  const cuuint32_t xb[5] = {8u, (cuuint32_t)HWD, (cuuint32_t)chunks_per_row,
+                            (cuuint32_t)(XMODE == 2 ? 2 * HROWS_LOAD : HROWS_LOAD), 1u};
+  const cuuint32_t xe[5] = {1u, 1u, 1u, 1u, 1u};
+  const CUresult rx = enc(&tmap_x, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 5, (void*)a.x, xd, xs, xb, xe,
+                          CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+                          CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (rx != CUDA_SUCCESS) {
+    set_last_error("conv_halo_wgrad: cuTensorMapEncodeTiled (x halo) failed (%d)", (int)rx);
+    return HB200_ERR_CUDA;
   }
   auto kern = conv_halo_wgrad_kernel<C, N, KH, KW, PAD, XMODE>;
   static int cache = 0;
@@ -1418,15 +818,6 @@ static int launch_wgrad_small(const grad_t* x, const grad_t* dy, float* dw, int 
 
 using namespace hb200;
 
-// halo loads by TMA (default) or by the cp.async gather kernel (HB200_NO_HALO_TMA=1, or hb200_set_halo_tma(0) from tests)
-static int g_halo_tma = getenv("HB200_NO_HALO_TMA") == nullptr ? 1 : 0;
-static int g_wgrad_xtma = getenv("HB200_WGRAD_XTMA") ? atoi(getenv("HB200_WGRAD_XTMA")) : 1;
-extern "C" int hb200_set_halo_tma(int enable) {
-  g_halo_tma = enable;   // 0 cp.async gather, 1 best per layer (default), 2 swizzled rows, 3 warp-specialised slabs, 4 both, 5 plain TMA slabs
-  return HB200_OK;
-}
-extern "C" int hb200_get_halo_tma(void) { return g_halo_tma; }
-
 /* which (C, N, k) combinations have a halo instantiation */
 extern "C" int hb200_conv_halo_supported(int c, int n, int k, int h, int w) {
   if (h % TH || w % TW) return 0;
@@ -1475,42 +866,12 @@ extern "C" int hb200_conv_halo(const hb200_bf16* x, const hb200_bf16* wimg, hb20
   a.B = batch; a.H = h; a.W = w; a.gn_groups = gn_groups > 0 ? gn_groups : 1;
   a.ntiles = batch * (h / TH) * (w / TW);
   cudaStream_t st = (cudaStream_t)stream;
-  // TMA-fed halo for every halo layer (no per-thread address / predicate work); HB200_NO_HALO_TMA=1 disables
-  const bool use_tma = g_halo_tma != 0;
-  // Loader per layer (hb200_set_halo_tma): 1 = the default per layer below (compare with tools/halo_bench.py):
-  //   64 / 32 channels: warp-specialised + swizzled pixel-row copies; the stem: warp-specialised slabs
-  // 2 / 3 / 4 / 5 force swizzled copies / warp-specialised slabs / warp-specialised swizzled / plain slabs everywhere.
-  if (g_halo_tma == 1 && k == 3 && c == 64)
+  if (k == 3 && c == 64)
     return mode == 0 ? launch_halo_ws<64, 64, 3, 3, 1, 0, 2, true>(a, st) : launch_halo_ws<64, 64, 3, 3, 1, 1, 2, true>(a, st);
-  if (g_halo_tma == 1 && k == 3 && c == 32)   // one CTA per SM: 18 KB of weights, 6 halo stages, 2 transpose buffers
+  if (k == 3 && c == 32)   // one CTA per SM: 18 KB of weights, 6 halo stages, 2 transpose buffers
     return mode == 0 ? launch_halo_ws<32, 32, 3, 3, 1, 0, 6, true>(a, st) : launch_halo_ws<32, 32, 3, 3, 1, 1, 6, true>(a, st);
-  if (g_halo_tma == 1 && k == 4 && mode == 0) return launch_halo_ws<16, 32, 4, 4, 2, 0, 6>(a, st);
-  if (g_halo_tma == 6 && k == 3 && c == 32)   // experiment: 2 stages, two CTAs per SM
-    return mode == 0 ? launch_halo_ws<32, 32, 3, 3, 1, 0, 2, true>(a, st) : launch_halo_ws<32, 32, 3, 3, 1, 1, 2, true>(a, st);
-  if (g_halo_tma == 4 && k == 3 && c == 32)
-    return mode == 0 ? launch_halo_ws<32, 32, 3, 3, 1, 0, 3, true>(a, st) : launch_halo_ws<32, 32, 3, 3, 1, 1, 3, true>(a, st);
-  if (g_halo_tma == 4 && k == 3 && c == 64)
-    return mode == 0 ? launch_halo_ws<64, 64, 3, 3, 1, 0, 2, true>(a, st) : launch_halo_ws<64, 64, 3, 3, 1, 1, 2, true>(a, st);
-  if (g_halo_tma == 3 && k == 3 && c == 32)
-    return mode == 0 ? launch_halo_ws<32, 32, 3, 3, 1, 0, 4>(a, st) : launch_halo_ws<32, 32, 3, 3, 1, 1, 4>(a, st);
-  if (g_halo_tma == 3 && k == 3 && c == 64)
-    return mode == 0 ? launch_halo_ws<64, 64, 3, 3, 1, 0, 5>(a, st) : launch_halo_ws<64, 64, 3, 3, 1, 1, 5>(a, st);
-  if (g_halo_tma == 3 && k == 4 && mode == 0) return launch_halo_ws<16, 32, 4, 4, 2, 0, 6>(a, st);
-  if (g_halo_tma == 2 && k == 3 && c == 32)
-    return mode == 0 ? launch_halo_sw<32, 32, 0>(a, st) : launch_halo_sw<32, 32, 1>(a, st);
-  if (g_halo_tma == 2 && k == 3 && c == 64)
-    return mode == 0 ? launch_halo_sw<64, 64, 0>(a, st) : launch_halo_sw<64, 64, 1>(a, st);
-  if (use_tma && k == 3 && c == 32)
-    return mode == 0 ? launch_halo_tma<32, 32, 3, 3, 1, 0>(a, st) : launch_halo_tma<32, 32, 3, 3, 1, 1>(a, st);
-  if (use_tma && k == 4 && mode == 0) return launch_halo_tma<16, 32, 4, 4, 2, 0>(a, st);
-  // 64-channel layers: single halo stage (72 KB of resident weights), the load replaces the cp.async gather's 1440
-  // copies per tile
-  if (use_tma && k == 3 && c == 64)
-    return mode == 0 ? launch_halo_tma<64, 64, 3, 3, 1, 0>(a, st) : launch_halo_tma<64, 64, 3, 3, 1, 1>(a, st);
-  if (k == 3 && c == 32) return mode == 0 ? launch_halo<32, 32, 3, 3, 1, 0>(a, st) : launch_halo<32, 32, 3, 3, 1, 1>(a, st);
-  if (k == 3 && c == 64) return mode == 0 ? launch_halo<64, 64, 3, 3, 1, 0>(a, st) : launch_halo<64, 64, 3, 3, 1, 1>(a, st);
   HB_CHECK_ARG(mode == 0, "conv_halo: the stem has no data gradient");
-  return launch_halo<16, 32, 4, 4, 2, 0>(a, st);
+  return launch_halo_ws<16, 32, 4, 4, 2, 0, 6>(a, st);
 }
 
 // accumulator of the space-to-depth weight gradient [((ky*2+kx)*4 + dy*2+dx) * ci + c][co] -> OIHW 3x3 gradient
@@ -1562,15 +923,7 @@ extern "C" int hb200_conv_halo_wgrad(const hb200_bf16* x, const hb200_bf16* dy, 
   a.B = batch; a.H = h; a.W = w;
   a.ntiles = batch * (h / TH) * (w / TW);
   cudaStream_t st = (cudaStream_t)stream;
-  // x halo: 0 = registers (C <= 32) / cp.async, 1 = one 5-D TMA box per tile (HB200_WGRAD_XTMA / hb200_set_wgrad_xtma)
-  if (g_wgrad_xtma) {
-    if (k == 3 && c == 32) return launch_halo_wgrad<32, 32, 3, 3, 1, 1>(a, st);
-    if (k == 3 && c == 64) return launch_halo_wgrad<64, 64, 3, 3, 1, 1>(a, st);
-    return launch_halo_wgrad<16, 32, 4, 4, 2, 1>(a, st);
-  }
-  if (k == 3 && c == 32) return launch_halo_wgrad<32, 32, 3, 3, 1>(a, st);
-  if (k == 3 && c == 64) return launch_halo_wgrad<64, 64, 3, 3, 1>(a, st);
-  return launch_halo_wgrad<16, 32, 4, 4, 2>(a, st);
+  if (k == 3 && c == 32) return launch_halo_wgrad<32, 32, 3, 3, 1, 1>(a, st);
+  if (k == 3 && c == 64) return launch_halo_wgrad<64, 64, 3, 3, 1, 1>(a, st);
+  return launch_halo_wgrad<16, 32, 4, 4, 2, 1>(a, st);
 }
-extern "C" int hb200_set_wgrad_xtma(int on) { g_wgrad_xtma = on ? 1 : 0; return HB200_OK; }
-extern "C" int hb200_get_wgrad_xtma(void) { return g_wgrad_xtma; }

@@ -2,18 +2,16 @@
 // visual_fc, the LSTM input projections and their data / weight gradients.
 //
 //   C[M,N] (f32) (+)= A[M,K] * B[K,N] (+ bias[N]) (ReLU)
-//   A(m,k) = a[m*a_ms + k*a_ks],  B(k,n) = b[k*b_ks + n*b_ns]   (one of the two strides of each == 1)
+//   A(m,k) = a[m*a_ms + k*a_ks],  B(k,n) = b[k*b_ks + n*b_ns]   (a_ks == b_ks == 1: both K-major)
 //
 // Precision: operands are fp32 in memory; the tensor core reads them as TF32 (10-bit mantissa,
 // the reference's own cuDNN-RNN precision on CUDA), accumulation is fp32 in the warpgroup's registers.
 //
-// wgmma reads tf32 operands K-major only: both operands are [rows][k] tiles in the 128-byte-swizzle layout, copied with
-// 16-byte cp.async (4 floats) or one TMA box per operand and chunk.
-// One MMA covers K = 8 (32 bytes); a chunk is K = 32 (4 MMAs); 3-stage cp.async ring as in conv.cu.
+// wgmma reads tf32 operands K-major only: both operands are [rows][k] tiles in the 128-byte-swizzle layout, one TMA box
+// per operand and chunk.  One MMA covers K = 8 (32 bytes); a chunk is K = 32 (4 MMAs).
 // Weight gradients (K = frames, tiny M x N tile grid) are split over K; the splits are summed in order (deterministic).
 #include <cuda.h>
 #include "common.cuh"
-#include <stdlib.h>
 #include <map>
 #include <mutex>
 #include "wgmma.cuh"
@@ -22,7 +20,7 @@ namespace hb200 {
 void count_launch(int n);
 using namespace wg;
 
-constexpr int GT_M = 128, GT_K = 32, GT_STAGES = 3;
+constexpr int GT_M = 128, GT_K = 32;
 
 constexpr uint32_t GT_A_HI = 8 * 1024;   // rows 0 -> 64 of a swizzled K-major tile
 
@@ -39,24 +37,8 @@ struct TgemmArgs {
   int vec4;   // c, ldc (and bias) allow 16-byte accesses
 };
 
-// load one K-major [ROWS x 32] operand tile (rows = m or n, zero-filled out of range)
-// vector = 4 consecutive k of one row; 8 vectors per row per chunk.  128-byte swizzle: 8 consecutive threads fetch the
-// 8 x 16 B of one row (a full 128-byte line) and write one swizzled shared-memory row (conflict free).
-__device__ __forceinline__ void tg_load(const float* __restrict__ p, long long s_mn, int mn0, int MN, int k0, int k_end,
-                                        uint32_t sdst, int rows) {
-  for (int v = threadIdx.x; v < rows * 8; v += 128) {
-    const int row = v >> 3, k4 = v & 7;
-    const int gm = mn0 + row, gk = k0 + k4 * 4;
-    const bool ok = gm < MN && gk + 3 < k_end;
-    const float* g = ok ? p + (long long)gm * s_mn + gk : p;
-    cp_async16(sdst + (uint32_t)((row >> 3) << 10) + (uint32_t)((row & 7) << 7) + (uint32_t)((k4 ^ (row & 7)) << 4),
-               g, ok);
-  }
-}
-
-// accumulator tile -> C: shared by the cp.async and the TMA kernels.  Plain launches add bias / accumulate / ReLU
-// here; split-K launches park their partial in the workspace for the ticketed reduction in split order (the same
-// sum every run).
+// accumulator tile -> C.  Plain launches add bias / accumulate / ReLU here; split-K launches park their partial in the
+// workspace for the ticketed reduction in split order (the same sum every run).
 template <int BN>
 __device__ __forceinline__ void tg_epilogue(const TgemmArgs& a, float (&acc_t)[BN], float* stage_buf, int m0, int n0) {
   const int tid = threadIdx.x;
@@ -146,62 +128,12 @@ __device__ __forceinline__ void tg_epilogue(const TgemmArgs& a, float (&acc_t)[B
   }
 }
 
-// NST = cp.async ring depth: 3 for the learner's many-CTA launches, deeper for the skinny (few CTAs, latency-bound) path
-template <int BN, int NST = GT_STAGES>
-__global__ void __launch_bounds__(128) tgemm_kernel(const TgemmArgs a) {
-  extern __shared__ __align__(16) uint8_t smem_raw[];
-  __shared__ float stage_buf[kStageFloats];
-  constexpr uint32_t kABytes = GT_M * GT_K * 4, kBBytes = BN * GT_K * 4, kStage = kABytes + kBBytes;
-  const uint32_t sbase = (smem_u32(smem_raw) + 1023u) & ~1023u;  // swizzle atoms are 1024-byte aligned
-  const int m0 = blockIdx.y * GT_M, n0 = blockIdx.x * BN;
-  const int k_begin = blockIdx.z * a.k_per_split;
-  const int k_end = min(a.K, k_begin + a.k_per_split);
-  const int nchunks = (k_end - k_begin + GT_K - 1) / GT_K;
-  if (nchunks <= 0) return;
-  float acc_t[BN];
-
-  auto load_chunk = [&](int c, int st) {
-    const uint32_t sa = sbase + st * kStage, sb = sa + kABytes;
-    const int k0 = k_begin + c * GT_K;
-    tg_load(a.a, a.a_ms, m0, a.M, k0, k_end, sa, GT_M);
-    tg_load(a.b, a.b_ns, n0, a.N, k0, k_end, sb, BN);
-  };
-#pragma unroll
-  for (int c = 0; c < NST - 1; ++c) {
-    if (c < nchunks) load_chunk(c, c);
-    cp_async_commit();
-  }
-  for (int c = 0; c < nchunks; ++c) {
-    const int st = c % NST;
-    cp_async_wait<NST - 2>();
-    fence_proxy_async_smem();
-    __syncthreads();
-    {
-      const uint32_t sa = sbase + st * kStage, sb = sa + kABytes;
-      wgmma_fence();
-#pragma unroll
-      for (int kk = 0; kk < GT_K / 8; ++kk)
-        mma128<BN, kTF32>(acc_t, make_smem_desc(sa + kk * 32, 16, 1024, kSwizzle128B), GT_A_HI,
-                          make_smem_desc(sb + kk * 32, 16, 1024, kSwizzle128B), (c > 0 || kk > 0) ? 1u : 0u);
-      wgmma_commit();
-    }
-    const int nc = c + NST - 1;
-    if (nc < nchunks) {
-      wgmma_wait<1>();   // the MMAs of chunk c-1 have read stage nc % NST
-      load_chunk(nc, nc % NST);
-    }
-    cp_async_commit();
-  }
-  wgmma_wait<0>();
-  tg_epilogue<BN>(a, acc_t, stage_buf, m0, n0);
-}
-
-// ---- TMA-fed variant ---------------------------------------------------------------------------------------------------
-// The cp.async kernel above spends far more issue slots per K chunk on 2048 LDGSTS + their addresses than the tensor core
-// needs for the chunk: the LSU work, not the tensor core, bounds it.  Here one thread issues two TMA box loads per chunk ([32 k] x [128 | BN
-// rows], SWIZZLE_128B = the K-major operand layout, out-of-range rows / k zero-filled by the TMA unit) into an NST-deep
-// ring ordered by full (transaction-count) barriers; the warpgroup refills a stage once wgmma.wait_group says the
-// MMAs that read it have completed.
+// ---- the GEMM kernel -----------------------------------------------------------------------------------------------------
+// One thread issues two TMA box loads per K chunk ([32 k] x [128 | BN rows], SWIZZLE_128B = the K-major operand layout,
+// out-of-range rows / k zero-filled by the TMA unit) into an NST-deep ring ordered by full (transaction-count) barriers;
+// the warpgroup refills a stage once wgmma.wait_group says the MMAs that read it have completed.  A 16-byte cp.async
+// gather of the same tiles spends far more issue slots per chunk on its 2048 LDGSTS and their addresses than the tensor
+// core needs for the chunk: the LSU work, not the tensor core, bounds it.
 template <int BN, int NST>
 __global__ void __launch_bounds__(128) tgemm_tma_kernel(const TgemmArgs a, const __grid_constant__ CUtensorMap tmap_a,
                                                         const __grid_constant__ CUtensorMap tmap_b) {
@@ -334,8 +266,6 @@ static int tg_tensor_map(CUtensorMap* tm, const float* p, long long rows, long l
   }
   return HB200_OK;
 }
-static int g_tgemm_tma = getenv("HB200_NO_TGEMM_TMA") ? 0 : 1;
-
 template <int BN, int NST>
 static int launch_tgemm_tma(const TgemmArgs& g, dim3 grid, cudaStream_t st) {
   CUtensorMap ta, tb;
@@ -352,28 +282,18 @@ static int launch_tgemm_tma(const TgemmArgs& g, dim3 grid, cudaStream_t st) {
   return HB200_OK;
 }
 
-extern "C" int hb200_set_tgemm_tma(int on) { g_tgemm_tma = on ? 1 : 0; return HB200_OK; }
-extern "C" int hb200_get_tgemm_tma(void) { return g_tgemm_tma; }
-
 extern "C" int hb200_tgemm(const float* a, long long a_ms, long long a_ks, const float* b, long long b_ks,
                            long long b_ns, float* c, long long ldc, const float* bias, int m, int n, int k,
                            int accumulate, int relu, hb200_stream_t stream) {
   HB_CHECK_ARG(a && b && c && m > 0 && n > 0 && k > 0, "tgemm: bad args");
   // wgmma reads tf32 operands K-major only -> callers transpose
   HB_CHECK_ARG(a_ks == 1 && b_ks == 1, "tgemm: both operands must be K-major (a_ks == 1, b_ks == 1)");
-  const int a_mn = (a_ks == 1) ? 0 : 1;   // k contiguous -> K-major
-  const int b_mn = (b_ks == 1) ? 0 : 1;
-  // 16-byte vector loads: leading dimensions / pointers must be multiples of 4 floats
-  const long long lda = a_mn ? a_ks : a_ms, ldb = b_mn ? b_ks : b_ns;
-  HB_CHECK_ARG(lda % 4 == 0 && ldb % 4 == 0 && ((uintptr_t)a & 15) == 0 && ((uintptr_t)b & 15) == 0,
+  // TMA: 16-byte aligned operands, row pitches multiples of 4 floats
+  HB_CHECK_ARG(a_ms % 4 == 0 && b_ns % 4 == 0 && ((uintptr_t)a & 15) == 0 && ((uintptr_t)b & 15) == 0,
                "tgemm: operands must be 16-byte aligned with leading dimensions that are multiples of 4");
-  HB_CHECK_ARG(k % 4 == 0 && (!a_mn || m % 4 == 0) && (!b_mn || n % 4 == 0), "tgemm: k (and mn-major extents) must be multiples of 4");
+  HB_CHECK_ARG(k % 4 == 0, "tgemm: k must be a multiple of 4");
   // N tile <= 128: a 128 x 128 fp32 accumulator is 128 registers per thread of the warpgroup
   int BN = n >= 128 ? 128 : (n >= 64 ? 64 : 32);
-  {
-    static const int forced = getenv("HB200_TGEMM_BN") ? atoi(getenv("HB200_TGEMM_BN")) : 0;
-    if ((forced == 32 || forced == 64 || forced == 128) && forced <= BN) BN = forced;
-  }
   HB_CHECK_ARG(n % 4 == 0, "tgemm: n must be a multiple of 4");
   TgemmArgs g;
   g.a = a; g.a_ms = a_ms; g.a_ks = a_ks; g.b = b; g.b_ks = b_ks; g.b_ns = b_ns; g.c = c; g.ldc = ldc; g.bias = bias;
@@ -381,10 +301,10 @@ extern "C" int hb200_tgemm(const float* a, long long a_ms, long long a_ks, const
   g.ws = nullptr; g.tickets = nullptr;
   g.vec4 = (ldc % 4 == 0 && ((uintptr_t)c & 15) == 0 && (!bias || ((uintptr_t)bias & 15) == 0)) ? 1 : 0;
   cudaStream_t st = (cudaStream_t)stream;
-  if (m <= GT_M && k >= 256 && cdiv(n, BN) < kNumSMs / 2 && !a_mn && !b_mn) {
+  if (m <= GT_M && k >= 256 && cdiv(n, BN) < kNumSMs / 2) {
     // one row tile (the actor: 64 frames): a handful of CTAs would each walk the whole K, one DRAM latency per
     // 32-wide chunk.  32-wide N tiles x K splits of >= 4 chunks put one CTA on every SM,
-    // each with a deep cp.async ring; partial tiles meet in an L2-resident workspace and the last CTA of each tile
+    // each with a deep TMA ring; partial tiles meet in an L2-resident workspace and the last CTA of each tile
     // reduces them in split order (8 KB per split).
     BN = 32;
     constexpr int kDeep = 6;   // 6 x (16 KB + 4 KB) stages
@@ -401,14 +321,7 @@ extern "C" int hb200_tgemm(const float* a, long long a_ms, long long a_ks, const
     }
     g.k_per_split = kps;
     dim3 grid(nt, 1, sp);
-    if (g_tgemm_tma) return launch_tgemm_tma<32, kDeep>(g, grid, st);
-    const size_t smem = (size_t)kDeep * (GT_M * GT_K * 4 + 32 * GT_K * 4) + 1024;
-    auto kern = tgemm_kernel<32, kDeep>;
-    HB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    kern<<<grid, 128, smem, st>>>(g);
-    HB_LAUNCH_OK();
-    count_launch(1);
-    return HB200_OK;
+    return launch_tgemm_tma<32, kDeep>(g, grid, st);
   }
   const long long tiles = (long long)cdiv(n, BN) * cdiv(m, GT_M);
   int splits = 1;
@@ -424,29 +337,11 @@ extern "C" int hb200_tgemm(const float* a, long long a_ms, long long a_ks, const
     if (rc) return rc;
   }
   dim3 grid(cdiv(n, BN), cdiv(m, GT_M), splits);
-  if (g_tgemm_tma && !a_mn && !b_mn) {
-    // ring depth: two CTAs per SM (3 x 32 KB stages) when there are enough tiles for that, else one CTA with a deep ring
-    const long long ctas = (long long)grid.x * grid.y * grid.z;
-    switch (BN) {
-      case 32: return launch_tgemm_tma<32, 4>(g, grid, st);
-      case 64: return launch_tgemm_tma<64, 4>(g, grid, st);
-      default: return ctas > kNumSMs ? launch_tgemm_tma<128, 3>(g, grid, st) : launch_tgemm_tma<128, 6>(g, grid, st);
-    }
-  }
-#define HB_TG(bn)                                                                                  \
-  {                                                                                                \
-    const size_t smem = (size_t)GT_STAGES * (GT_M * GT_K * 4 + bn * GT_K * 4) + 1024;              \
-    auto kern = tgemm_kernel<bn>;                                                                  \
-    HB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));   \
-    kern<<<grid, 128, smem, st>>>(g);                                                              \
-  }
+  // ring depth: two CTAs per SM (3 x 32 KB stages) when there are enough tiles for that, else one CTA with a deep ring
+  const long long ctas = (long long)grid.x * grid.y * grid.z;
   switch (BN) {
-    case 32: HB_TG(32); break;
-    case 64: HB_TG(64); break;
-    default: HB_TG(128); break;
+    case 32: return launch_tgemm_tma<32, 4>(g, grid, st);
+    case 64: return launch_tgemm_tma<64, 4>(g, grid, st);
+    default: return ctas > kNumSMs ? launch_tgemm_tma<128, 3>(g, grid, st) : launch_tgemm_tma<128, 6>(g, grid, st);
   }
-#undef HB_TG
-  HB_LAUNCH_OK();
-  count_launch(1);
-  return HB200_OK;
 }

@@ -1,8 +1,8 @@
 // hb200 -- TMA halo load probe (pins the halo kernels' tensor-map encoding; not on the product path).
 //
-// Next step for the halo convolutions (NOTES_NEXT.md item 4): replace the per-thread zero-filling cp.async gather of the
-// (TH+KH-1) x (TW+KW-1) input halo -- ~6 copies per thread, each with its own address and bounds predicate, the reason
-// conv_halo_kernel<32,32> is issue-bound -- by C/8 `cp.async.bulk.tensor.4d` box copies issued by ONE thread: box =
+// The halo convolutions load the (TH+KH-1) x (TW+KW-1) input halo not by a per-thread zero-filling cp.async gather --
+// ~6 copies per thread, each with its own address and bounds predicate, which made the 32-channel layer issue-bound --
+// but by C/8 `cp.async.bulk.tensor.4d` box copies issued by ONE thread: box =
 // {8 channels, halo width, halo height, 1 frame} of the NHWC tensor, out-of-bounds rows / columns zero-filled by the TMA
 // unit (that is the conv padding), completion signalled on an mbarrier.  The box lands as [hy][hx][8 ch] = one 16-byte
 // vector per pixel, i.e. exactly one channel-chunk slab of the no-swizzle K-major operand layout the wgmma shared-

@@ -442,22 +442,20 @@ class EncoderEngine:
         assert self.comp.out_hw == tuple(enc.output_shape[1:]), (self.comp.out_hw, enc.output_shape)
         self.convs: List[_Conv] = ([self.stem] + [c for convs, cd in self.blocks for c in convs + ([cd] if cd else [])]
                                    + [self.comp])
-        if not os.environ.get("HB200_NO_HALO"):
-            for c in self.convs:
-                if c is self.stem:
-                    c.stem_s2d = (allow_s2d and c.k == 7 and c.stride == 2 and c.pad == 3 and c.ci_real <= 4 and
-                                  self.hp % 2 == 0 and self.wp_ % 2 == 0 and
-                                  ops.conv_halo_supported(16, c.co, 4, c.out_hw[0], c.out_hw[1]))
-                elif c.k == 3 and c.stride == 1 and c.pad == 1:
-                    c.halo = ops.conv_halo_supported(c.ci, c.co, 3, c.in_hw[0], c.in_hw[1])
-                    c.halo_w = ops.conv_halo_wgrad_supported(c.ci, c.co, 3, c.in_hw[0], c.in_hw[1])
-            if not os.environ.get("HB200_NO_CONV_S2"):
-                for convs, cd in self.blocks:   # stride-2 block entry: 3x3 s2 conv + 1x1 s2 downsample in one kernel
-                    c = convs[0]
-                    if (cd is not None and c.k == 3 and c.stride == 2 and c.pad == 1 and cd.k == 1 and cd.stride == 2
-                            and cd.pad == 0 and c.conv_groups == 1 and cd.conv_groups == 1 and c.ci == c.ci_real
-                            and ops.conv_s2_supported(c.ci, c.co, cd.co, c.in_hw[0], c.in_hw[1])):
-                        c.s2_pair, cd.s2_main = cd, c
+        for c in self.convs:
+            if c is self.stem:
+                c.stem_s2d = (allow_s2d and c.k == 7 and c.stride == 2 and c.pad == 3 and c.ci_real <= 4 and
+                              self.hp % 2 == 0 and self.wp_ % 2 == 0 and
+                              ops.conv_halo_supported(16, c.co, 4, c.out_hw[0], c.out_hw[1]))
+            elif c.k == 3 and c.stride == 1 and c.pad == 1:
+                c.halo = ops.conv_halo_supported(c.ci, c.co, 3, c.in_hw[0], c.in_hw[1])
+                c.halo_w = ops.conv_halo_wgrad_supported(c.ci, c.co, 3, c.in_hw[0], c.in_hw[1])
+        for convs, cd in self.blocks:   # stride-2 block entry: 3x3 s2 conv + 1x1 s2 downsample in one kernel
+            c = convs[0]
+            if (cd is not None and c.k == 3 and c.stride == 2 and c.pad == 1 and cd.k == 1 and cd.stride == 2
+                    and cd.pad == 0 and c.conv_groups == 1 and cd.conv_groups == 1 and c.ci == c.ci_real
+                    and ops.conv_s2_supported(c.ci, c.co, cd.co, c.in_hw[0], c.in_hw[1])):
+                c.s2_pair, cd.s2_main = cd, c
         self._ws = {}
         self._dev = None
         self._packed_key = None

@@ -203,7 +203,7 @@ int hb200_conv_wgrad(const hb200_bf16* x, const hb200_bf16* dy, float* dw_acc,
                      const hb200_conv_shape* s, hb200_stream_t stream);
 /* f32 OIHW [Co,Ci_real,kh,kw] -> bf16 [Co][(r,s,ci) padded] (ci_pad >= ci_real, zero filled),
  * and the transposed pack [Ci_pad][(r,s,co) padded] used by dgrad.  Both are stored as
- * ready-to-copy shared-memory tile images (see hb200_set_umma_layout). */
+ * ready-to-copy shared-memory tile images (128-byte swizzle, K-major). */
 int hb200_pack_conv_weight(const float* w_oihw, hb200_bf16* w_packed, hb200_bf16* w_packed_t,
                            int co, int ci_real, int ci_pad, int kh, int kw, hb200_stream_t stream);
 /* dw_acc f32 [(r,s,ci_pad)][Co] -> f32 OIHW grad [Co,Ci_real,kh,kw] (overwrite) */
@@ -213,10 +213,6 @@ int hb200_unpack_conv_wgrad(const float* dw_acc, float* dw_oihw, int co, int ci_
 /* number of bf16 elements of a packed weight image with n_rows GEMM rows and
  * kh*kw*k_channels reduction length (padded to the 64-element K chunk) */
 size_t hb200_packed_weight_elems(int n_rows, int k_channels, int kh, int kw);
-/* shared-memory operand layout used by the conv kernels AND the weight images
- * (0 = no-swizzle interleaved core matrices, 1 = 128-byte swizzle); set before packing. */
-int hb200_set_umma_layout(int layout);
-int hb200_get_umma_layout(void);
 
 /* ---- "halo" convolutions: stride-1 k x k layers (k=3 pad 1; k=4 = the space-to-depth stem) ----------
  * Each CTA loads the input halo of a 16x8 output tile once and addresses every filter tap with a
@@ -230,16 +226,6 @@ int hb200_pack_halo_weight(const float* w_oihw, hb200_bf16* img, int co, int ci_
 int hb200_conv_halo(const hb200_bf16* x, const hb200_bf16* wimg, hb200_bf16* y, const hb200_bf16* addend,
                     double* gn_stats, int gn_groups, int batch, int h, int w, int c, int n, int k, int mode,
                     hb200_stream_t stream);
-/* Halo loader of the forward / dgrad halo kernels: 0 = zero-filling cp.async gather (also HB200_NO_HALO_TMA=1 in the
- * environment), 1 = the measured best TMA variant per layer (default), 2 = TMA copies of whole pixel rows into the
- * swizzled K-major layout, 3 = warp-specialised pipeline over 16-byte channel slabs, 4 = warp-specialised + swizzled
- * rows, 5 = plain TMA slabs.  All are kept parity-tested (tests/test_gpu_kernels.py::test_conv_halo_3x3). */
-int hb200_set_halo_tma(int mode);
-int hb200_get_halo_tma(void);
-/* x halo of the halo weight-gradient kernels: 0 = register staging / cp.async, 1 = one 5-D TMA box per tile (default;
- * HB200_WGRAD_XTMA=0 in the environment selects 0 at load time) */
-int hb200_set_wgrad_xtma(int on);
-int hb200_get_wgrad_xtma(void);
 
 /* 1 if hb200_conv_halo_wgrad serves this 3x3 / stem shape: the hb200_conv_halo_supported shapes plus the small-image
  * layers (8x8 and 4x4 inputs, c % 32 == 0, n % 128 == 0: layer3 / layer4 / compression of
@@ -257,10 +243,6 @@ int hb200_conv_halo_wgrad_supported(int c, int n, int k, int h, int w);
  *            packed with mode 1 (c = NA + NB, n = C).
  * Supported: C = 32, NA = NB = 64, H % 32 == 0, W % 16 == 0 (layer2.0 of the resnet18 encoder at 256x256 input). */
 int hb200_conv_s2_supported(int c, int na, int nb, int h, int w);
-/* forward / dgrad variant: 1 (default) = warp-specialised pipeline over swizzled 128-byte pixel-row copies, 0 = one-thread
- * pipeline over 16-byte channel slabs (HB200_NO_CONV_S2_WS=1 in the environment selects 0 at load time) */
-int hb200_set_conv_s2_ws(int on);
-int hb200_get_conv_s2_ws(void);
 /* weight gradient of the 3x3 stride-2 branch over the same space-to-depth view (x halo = one 5-D TMA box per tile):
  * x bf16 [B,H,W,C] (twin of the forward input), dy bf16 [B,H/2,W/2,N]; dw_acc f32 [16*C][N], pre-zeroed, rows
  * ((ky*2+kx)*4 + dy*2+dx)*C + c; hb200_unpack_s2_wgrad writes the 9 real taps as OIHW.  C = 32, N = 64. */
@@ -390,10 +372,6 @@ int hb200_sgemm(const float* a, long long a_ms, long long a_ks, const float* b, 
 int hb200_tgemm(const float* a, long long a_ms, long long a_ks, const float* b, long long b_ks, long long b_ns,
                 float* c, long long ldc, const float* bias, int m, int n, int k, int accumulate, int relu,
                 hb200_stream_t stream);
-/* operand feed of hb200_tgemm: 1 (default) = TMA box loads, 0 = the 16-byte cp.async gather (kept for A/B tests;
- * environment HB200_NO_TGEMM_TMA=1 selects it at load time) */
-int hb200_set_tgemm_tma(int on);
-int hb200_get_tgemm_tma(void);
 /* dst[c,r] = src[r,c] (fp32): feeds hb200_tgemm K-major operands for the data / weight gradient GEMMs */
 int hb200_transpose_f32(const float* src, long long ld_src, float* dst, long long ld_dst, int rows, int cols,
                         hb200_stream_t stream);

@@ -370,18 +370,8 @@ def test_conv_fwd_dgrad_wgrad(hb, case):
                                    atol=2e-2 * max(1.0, dx_ref.abs().max().item()))
 
 
-@pytest.fixture(params=[1, 0], ids=["ws_swizzled", "slabs"])
-def s2_variant(hb, request):
-    """forward / dgrad of the stride-2 block entry: warp-specialised swizzled pixel-row copies (default) or 16-byte slabs"""
-    lib = hb.load()
-    prev = lib.hb200_get_conv_s2_ws()
-    lib.hb200_set_conv_s2_ws(request.param)
-    yield request.param
-    lib.hb200_set_conv_s2_ws(prev)
-
-
 @pytest.mark.parametrize("B,H,W", [(3, 32, 32), (2, 64, 16), (160, 32, 32)])
-def test_conv_s2_block_entry(hb, s2_variant, B, H, W):
+def test_conv_s2_block_entry(hb, B, H, W):
     """conv_s2.cu: 3x3 stride-2 conv + 1x1 stride-2 downsample conv of one input in one launch (forward with both
     GroupNorm sums, and the summed data gradient) over the TMA space-to-depth view, vs torch convolutions."""
     from habitat_lab_b200 import ops
@@ -444,31 +434,8 @@ def test_conv_s2_block_entry(hb, s2_variant, B, H, W):
 HALO_CASES = [(3, 32, 32, 32, 32), (2, 16, 16, 64, 64), (5, 16, 8, 32, 32), (600, 32, 32, 32, 32)]
 
 
-@pytest.fixture(params=[1, 0, 2, 3, 4, 5],
-                ids=["default", "cp_async", "tma_swizzled", "tma_warp_specialised", "tma_ws_swizzled", "tma_slabs"])
-def halo_loader(hb, request):
-    """the halo load paths of the forward / dgrad halo kernels: the per-layer default, the cp.async gather, TMA copies of
-    whole pixel rows into the swizzled K-major layout (three pre-shifted copies per tile), the warp-specialised pipeline
-    (slabs / swizzled rows) and plain TMA box copies of 16-byte channel slabs"""
-    lib = hb.load()
-    prev = lib.hb200_get_halo_tma()
-    lib.hb200_set_halo_tma(request.param)
-    yield request.param
-    lib.hb200_set_halo_tma(prev)
-
-
-@pytest.fixture(params=[0, 1], ids=["x_regs", "x_tma"])
-def wgrad_x(hb, request):
-    """x halo of the halo weight-gradient kernels: register staging / cp.async, or one 5-D TMA box per tile"""
-    lib = hb.load()
-    prev = lib.hb200_get_wgrad_xtma()
-    lib.hb200_set_wgrad_xtma(request.param)
-    yield request.param
-    lib.hb200_set_wgrad_xtma(prev)
-
-
 @pytest.mark.parametrize("B,H,W,C,N", HALO_CASES)
-def test_conv_halo_3x3(hb, halo_loader, wgrad_x, B, H, W, C, N):
+def test_conv_halo_3x3(hb, B, H, W, C, N):
     """halo kernels (one input load per tile, taps by descriptor shift) vs fp32 conv of the same rounded operands"""
     from habitat_lab_b200 import ops
 
@@ -537,7 +504,7 @@ def test_conv_halo_wgrad_small_images(hb, B, HW, C, N):
 
 
 @pytest.mark.parametrize("B,Hp,Wp", [(2, 128, 128), (3, 64, 32)])
-def test_conv_halo_stem_s2d(hb, halo_loader, wgrad_x, B, Hp, Wp):
+def test_conv_halo_stem_s2d(hb, B, Hp, Wp):
     """7x7 stride-2 pad-3 stem == 4x4 stride-1 conv over the space-to-depth input"""
     from habitat_lab_b200 import ops
 
@@ -797,25 +764,16 @@ def test_sgemm_linear(hb, M, N, K):
     torch.testing.assert_close(db, dy.sum(0), rtol=1e-4, atol=1e-3)
 
 
-@pytest.fixture(params=[1, 0], ids=["tma", "cp_async"])
-def tgemm_feed(hb, request):
-    """both operand feeds of hb200_tgemm: TMA box loads (default) and the 16-byte cp.async gather"""
-    lib = hb.load()
-    prev = lib.hb200_get_tgemm_tma()
-    lib.hb200_set_tgemm_tma(request.param)
-    yield request.param
-    lib.hb200_set_tgemm_tma(prev)
-
-
 @pytest.mark.parametrize("M,N,K", [(4096, 512, 2048), (4096, 2048, 576), (128, 64, 64), (260, 36, 100),
                                    # one row tile (the actor's batches): deterministic split-K through the workspace
                                    (64, 512, 2048), (64, 2048, 576), (64, 2048, 512), (3, 36, 260), (128, 512, 4096),
                                    # SimpleCNN's Linear(flatten, 512): RGB-D 256x256 (K = 25088) at the actor's 6 frames
                                    # and a 256-frame minibatch, RGB 84x116 (K = 2464) at 128 frames
                                    (6, 512, 25088), (256, 512, 25088), (128, 512, 2464)])
-def test_tgemm_tf32(hb, tgemm_feed, M, N, K):
-    """wgmma tf32 dense layers: forward (K-major x K-major), data gradient (K-major x N-major) and
-    split-K weight gradient (M-major x N-major) vs fp64; tolerance = TF32 operand rounding (2^-11 relative)."""
+def test_tgemm_tf32(hb, M, N, K):
+    """wgmma tf32 dense layers vs fp64: forward x @ w^T, data gradient dy @ w and split-K weight gradient dy^T @ x, the
+    gradients' operands transposed on the device so that both are K-major (the only form hb200_tgemm takes);
+    tolerance = TF32 operand rounding (2^-11 relative)."""
     from habitat_lab_b200 import ops
 
     torch.manual_seed(M + N + K)
@@ -968,7 +926,7 @@ def test_gru_masked_recurrence(hb, T, n, H, D):
     torch.testing.assert_close(db_hh.cpu(), sdr["rnn.bias_hh_l0"].grad, rtol=1e-3, atol=1e-3)
 
 
-def test_tgemm_skinny_split_k_is_deterministic_and_accumulates(hb, tgemm_feed):
+def test_tgemm_skinny_split_k_is_deterministic_and_accumulates(hb):
     """The one-row-tile path reduces its K splits in split order (no atomics): repeated launches are bit-identical, and
     accumulate / ReLU / bias run once, in the reducing CTA."""
     from habitat_lab_b200 import ops

@@ -2,9 +2,8 @@
 
 conv_halo_ws_kernel hands the tiles of a CTA alternately to two consumer warpgroups, so a CTA with an odd number of
 tiles, or with a single one, leaves the second warpgroup with one tile fewer or none.  Its grid is one CTA per SM (132)
-for the 32- and 64-channel layers by default and two per SM for loader 6 and the stem, so the cases put the tile count
-below the grid, at one and two tiles per CTA, and one tile past a multiple of the grid.  The 16 x 8 images are one
-128-pixel tile per frame.
+for the 32- and 64-channel layers and two per SM for the stem, so the cases put the tile count below the grid, at one
+and two tiles per CTA, and one tile past a multiple of the grid.  The 16 x 8 images are one 128-pixel tile per frame.
 
 conv_igemm_kernel runs two CTAs per SM at the full 128-wide N tile; the cases put its CTA count below the SM count
 (without the narrow N slices the actor's launches get), at exactly one and two CTAs per SM, one past that, and stride-2
@@ -47,32 +46,21 @@ def _check_stats(stats, y_ref, B, G):
     torch.testing.assert_close(stats[..., 1].float(), (yg * yg).sum(-1), rtol=1e-3, atol=2e-2)
 
 
-@pytest.fixture
-def halo_mode(hb, request):
-    lib = hb.load()
-    prev = lib.hb200_get_halo_tma()
-    lib.hb200_set_halo_tma(request.param)
-    yield request.param
-    lib.hb200_set_halo_tma(prev)
-
-
 HALO_TILE_CASES = [
-    # loader, B, H, W, C   (one tile per 16 x 8 frame; default grid 132 CTAs, loader 6 grid 264)
-    (1, 7, 16, 8, 32),               # fewer tiles than SMs, one tile per CTA: warpgroup 1 idle
-    (1, 131, 16, 8, 32),             # odd, below the grid
-    (1, SMS, 16, 8, 32),             # exactly one tile per CTA
-    (1, 2 * SMS, 16, 8, 32),         # exactly two: one per warpgroup
-    (1, 2 * SMS + 1, 16, 8, 32),     # one CTA with three tiles
-    (1, 5 * SMS + 3, 16, 8, 32),     # odd tile count per CTA (5 or 6), ring of 6 stages wraps
-    (1, 2 * SMS + 1, 16, 8, 64),     # 64 channels, 2-stage ring
-    (1, 37, 32, 32, 32),             # 296 tiles on 132 CTAs
-    (6, 2 * 2 * SMS + 1, 16, 8, 32),  # two CTAs per SM, 2-stage ring
-    (3, 3 * SMS + 1, 16, 8, 64),     # 16-byte slabs, 5-stage ring
+    # B, H, W, C   (one tile per 16 x 8 frame; grid 132 CTAs)
+    (7, 16, 8, 32),               # fewer tiles than SMs, one tile per CTA: warpgroup 1 idle
+    (131, 16, 8, 32),             # odd, below the grid
+    (SMS, 16, 8, 32),             # exactly one tile per CTA
+    (2 * SMS, 16, 8, 32),         # exactly two: one per warpgroup
+    (2 * SMS + 1, 16, 8, 32),     # one CTA with three tiles
+    (5 * SMS + 3, 16, 8, 32),     # odd tile count per CTA (5 or 6), ring of 6 stages wraps
+    (2 * SMS + 1, 16, 8, 64),     # 64 channels, 2-stage ring
+    (37, 32, 32, 32),             # 296 tiles on 132 CTAs
 ]
 
 
-@pytest.mark.parametrize("halo_mode,B,H,W,C", HALO_TILE_CASES, indirect=["halo_mode"])
-def test_conv_halo_ws_tile_counts(hb, halo_mode, B, H, W, C):
+@pytest.mark.parametrize("B,H,W,C", HALO_TILE_CASES)
+def test_conv_halo_ws_tile_counts(hb, B, H, W, C):
     from habitat_lab_b200 import ops
 
     N, G = C, 16

@@ -20,7 +20,6 @@ CSRC = os.path.join(ROOT, "habitat-lab_b200", "csrc")
 ATOMICS_ALLOWED = {
     "conv_igemm_kernel": "fp64 GroupNorm sum / sum of squares of fp32 accumulator partials (exact, see above)",
     "halo_gn_stats_chunk": "fp64 GroupNorm statistics of fp32 partials (exact, see above)",
-    "conv_halo_kernel": "fp64 GroupNorm statistics of fp32 partials (exact, see above)",
     "s2_gn_stats_chunk": "fp64 GroupNorm statistics of fp32 partials (exact, see above)",
     "prep_stats_kernel": "fp64 RunningMeanAndVar sums of fp32 pooled pixels (exact, see above)",
     "prep_generic_kernel": "fp64 RunningMeanAndVar sums of fp32 pooled pixels (exact, see above)",

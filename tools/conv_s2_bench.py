@@ -59,12 +59,6 @@ def gather_dgrad():
     ops.conv_dgrad(dyb, wtd, dx, s_d, addend=dx)
 
 
-for ws in (1, 0):
-    hb.load().hb200_set_conv_s2_ws(ws)
-    tf_ = timed(lambda: ops.conv_s2_fwd(x, img, ya, yb, B, H, W, C, NA, NB, stats_a=sa, groups_a=G, stats_b=sb, groups_b=G))
-    td_ = timed(lambda: ops.conv_s2_dgrad(dya, dyb, img_t, dx, B, H, W, C, NA, NB))
-    print(f"B={B}: conv_s2 variant {'ws + swizzled rows' if ws else 'slabs'}: forward {tf_:7.1f} us  dgrad {td_:7.1f} us")
-hb.load().hb200_set_conv_s2_ws(1)
 print(f"B={B}: forward  fused {timed(lambda: ops.conv_s2_fwd(x, img, ya, yb, B, H, W, C, NA, NB, stats_a=sa, groups_a=G, stats_b=sb, groups_b=G)):7.1f} us"
       f"   gather (2 launches) {timed(gather_fwd):7.1f} us")
 print(f"B={B}: dgrad    fused {timed(lambda: ops.conv_s2_dgrad(dya, dyb, img_t, dx, B, H, W, C, NA, NB)):7.1f} us"

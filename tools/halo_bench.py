@@ -1,5 +1,5 @@
-"""3x3 stride-1 halo convolutions of the resnet18 encoder at 4096 frames, forward and dgrad, per halo load path
-(hb200_set_halo_tma: 0 cp.async, 1 TMA slabs, 2 TMA swizzled pixel rows)."""
+"""Halo convolutions of the resnet18 encoder at 4096 frames: the 3x3 stride-1 layers (forward, dgrad, weight gradient)
+and the space-to-depth stem (forward, weight gradient)."""
 import os
 import sys
 
@@ -11,7 +11,7 @@ import habitat_lab_b200 as hb  # noqa: E402
 from habitat_lab_b200 import ops  # noqa: E402
 
 dev = torch.device("cuda:0")
-lib = hb.load()
+hb.load()
 B = int(sys.argv[1]) if len(sys.argv) > 1 else 4096
 
 
@@ -40,13 +40,10 @@ for H, C in ((32, 32), (16, 64)):
     dx = torch.empty_like(dy)
     st = torch.zeros(B, 16, 2, device=dev, dtype=torch.float64)
     flop = 2.0 * B * H * H * C * C * 9
-    for mode in (6, 4, 3, 1, 2, 0, 5):
-        lib.hb200_set_halo_tma(mode)
-        tf = timed(lambda: ops.conv_halo(x, wh, y, B, H, H, C, C, 3, 0, gn_stats=st, gn_groups=16))
-        td = timed(lambda: ops.conv_halo(dy, wt, dx, B, H, H, C, C, 3, 1))
-        print(f"{C}ch {H}x{H} B={B} loader={mode}: fwd {tf:7.1f} us ({flop / tf / 1e6:6.1f} TF/s)  dgrad {td:7.1f} us "
-              f"({flop / td / 1e6:6.1f} TF/s)")
-lib.hb200_set_halo_tma(1)
+    tf = timed(lambda: ops.conv_halo(x, wh, y, B, H, H, C, C, 3, 0, gn_stats=st, gn_groups=16))
+    td = timed(lambda: ops.conv_halo(dy, wt, dx, B, H, H, C, C, 3, 1))
+    print(f"{C}ch {H}x{H} B={B}: fwd {tf:7.1f} us ({flop / tf / 1e6:6.1f} TF/s)  dgrad {td:7.1f} us "
+          f"({flop / td / 1e6:6.1f} TF/s)")
 
 # stem forward (7x7 s2 as 4x4 s1 over the space-to-depth input, 16 -> 32 channels @ 64x64)
 x = torch.randn(B, 64, 64, 16, device=dev).half()
@@ -55,27 +52,19 @@ wh = torch.empty(16 * 16 * 32, device=dev, dtype=torch.float16)
 ops.pack_halo_weight(w, wh, 16, 32, 4, 2)
 y = torch.empty(B, 64, 64, 32, device=dev, dtype=torch.float16)
 st = torch.zeros(B, 16, 2, device=dev, dtype=torch.float64)
-for mode in (3, 1, 0):
-    lib.hb200_set_halo_tma(mode)
-    t = timed(lambda: ops.conv_halo(x, wh, y, B, 64, 64, 16, 32, 4, 0, gn_stats=st, gn_groups=16))
-    t0 = timed(lambda: ops.conv_halo(x, wh, y, B, 64, 64, 16, 32, 4, 0))
-    print(f"stem 64x64 B={B} loader={mode}: fwd {t:7.1f} us   (without the GroupNorm sums: {t0:7.1f} us)")
-lib.hb200_set_halo_tma(1)
+t = timed(lambda: ops.conv_halo(x, wh, y, B, 64, 64, 16, 32, 4, 0, gn_stats=st, gn_groups=16))
+t0 = timed(lambda: ops.conv_halo(x, wh, y, B, 64, 64, 16, 32, 4, 0))
+print(f"stem 64x64 B={B}: fwd {t:7.1f} us   (without the GroupNorm sums: {t0:7.1f} us)")
 
-# weight gradients: x halo through registers / cp.async vs one 5-D TMA box per tile
+# weight gradients (x halo and dy tile by TMA)
 for H, C in ((32, 32), (16, 64)):
     x = torch.randn(B, H, H, C, device=dev).bfloat16()
     dy = torch.randn(B, H, H, C, device=dev).bfloat16()
     acc = torch.zeros(9 * C, C, device=dev)
-    for xt in (0, 1):
-        lib.hb200_set_wgrad_xtma(xt)
-        t = timed(lambda: ops.conv_halo_wgrad(x, dy, acc, B, H, H, C, C, 3))
-        print(f"{C}ch {H}x{H} B={B} wgrad x_tma={xt}: {t:7.1f} us")
+    t = timed(lambda: ops.conv_halo_wgrad(x, dy, acc, B, H, H, C, C, 3))
+    print(f"{C}ch {H}x{H} B={B} wgrad: {t:7.1f} us")
 x = torch.randn(B, 64, 64, 16, device=dev).bfloat16()
 dy = torch.randn(B, 64, 64, 32, device=dev).bfloat16()
 acc = torch.zeros(16 * 16, 32, device=dev)
-for xt in (0, 1):
-    lib.hb200_set_wgrad_xtma(xt)
-    t = timed(lambda: ops.conv_halo_wgrad(x, dy, acc, B, 64, 64, 16, 32, 4))
-    print(f"stem 16ch(s2d) 64x64 B={B} wgrad x_tma={xt}: {t:7.1f} us")
-lib.hb200_set_wgrad_xtma(0)
+t = timed(lambda: ops.conv_halo_wgrad(x, dy, acc, B, 64, 64, 16, 32, 4))
+print(f"stem 16ch(s2d) 64x64 B={B} wgrad: {t:7.1f} us")

@@ -1,4 +1,4 @@
-"""One forward + one dgrad launch of a halo conv for ncu: `python tools/halo_probe.py C H loader_mode`."""
+"""One forward + one dgrad launch of a halo conv for ncu: `python tools/halo_probe.py C H`."""
 import os
 import sys
 
@@ -9,11 +9,10 @@ sys.path.insert(0, ROOT)
 import habitat_lab_b200 as hb  # noqa: E402
 from habitat_lab_b200 import ops  # noqa: E402
 
-C, H, mode = int(sys.argv[1]), int(sys.argv[2]), int(sys.argv[3])
+C, H = int(sys.argv[1]), int(sys.argv[2])
 B = 4096
 dev = torch.device("cuda:0")
-lib = hb.load()
-lib.hb200_set_halo_tma(mode)
+hb.load()
 x = torch.randn(B, H, H, C, device=dev).half()
 dy = torch.randn(B, H, H, C, device=dev).bfloat16()
 w = torch.randn(C, C, 3, 3, device=dev) * 0.05

@@ -1,5 +1,5 @@
 """TF32 dense layers of config #2 (visual_fc, LSTM input projections: forward, data gradient, weight gradient) through
-hb200_tgemm with both operand feeds: CUDA-event time per launch and TFLOP/s."""
+hb200_tgemm: CUDA-event time per launch and TFLOP/s."""
 import os
 import sys
 
@@ -11,7 +11,7 @@ import habitat_lab_b200 as hb  # noqa: E402
 from habitat_lab_b200 import ops  # noqa: E402
 
 dev = torch.device("cuda:0")
-lib = hb.load()
+hb.load()
 torch.manual_seed(0)
 M = int(sys.argv[1]) if len(sys.argv) > 1 else 4096
 
@@ -36,12 +36,9 @@ for name, N, K in (("visual_fc", 512, 2048), ("lstm_l0_ih", 2048, 576), ("lstm_l
     dy = torch.randn(M, N, device=dev)
     dx = torch.empty(M, K, device=dev)
     dw = torch.zeros(N, K, device=dev)
-    for feed in (1, 0):
-        lib.hb200_set_tgemm_tma(feed)
-        t_f = timed(lambda: ops.linear_fwd(x, w, b, out, relu=True, tf32=True))
-        t_d = timed(lambda: ops.linear_bwd_input(dy, w, dx, tf32=True))
-        t_w = timed(lambda: ops.linear_bwd_weight(dy, x, dw, accumulate=True, tf32=True))
-        fl = 2.0 * M * N * K
-        print(f"{name:11s} M={M} N={N} K={K} feed={'tma' if feed else 'cp.async'}: fwd {t_f * 1e3:7.1f} us "
-              f"({fl / t_f / 1e9:6.1f} TF/s)  dgrad(+transpose) {t_d * 1e3:7.1f} us  wgrad(+transposes) {t_w * 1e3:7.1f} us")
-lib.hb200_set_tgemm_tma(1)
+    t_f = timed(lambda: ops.linear_fwd(x, w, b, out, relu=True, tf32=True))
+    t_d = timed(lambda: ops.linear_bwd_input(dy, w, dx, tf32=True))
+    t_w = timed(lambda: ops.linear_bwd_weight(dy, x, dw, accumulate=True, tf32=True))
+    fl = 2.0 * M * N * K
+    print(f"{name:11s} M={M} N={N} K={K}: fwd {t_f * 1e3:7.1f} us ({fl / t_f / 1e9:6.1f} TF/s)  "
+          f"dgrad(+transpose) {t_d * 1e3:7.1f} us  wgrad(+transposes) {t_w * 1e3:7.1f} us")

@@ -13,6 +13,8 @@ _LAZY = {
     "PointNavResNetPolicy": ("rl.resnet_policy", "PointNavResNetPolicy"),
     "PointNavBaselinePolicy": ("rl.policy", "PointNavBaselinePolicy"),
     "RolloutObservations": ("rl.resnet_policy", "RolloutObservations"),
+    "GaussianNet": ("rl.resnet_policy", "GaussianNet"),
+    "ActionDistributionConfig": ("rl.resnet_policy", "ActionDistributionConfig"),
     "PPO": ("rl.ppo", "PPO"),
     "DDPPO": ("rl.ppo", "DDPPO"),
     "FusedAdam": ("rl.ppo", "FusedAdam"),

@@ -31,6 +31,9 @@ SIGNATURES = {
     "hb200_adv_normalize": ("i", "plppip"),
     "hb200_ppo_loss_workspace_bytes": ("z", "iii"),
     "hb200_ppo_loss": ("i", "ppppppppppp" + "iii" + "fff" + "ii" + "ppp" + "ppppp" + "ppp"),
+    "hb200_gaussian_act": ("i", "ppppppp" + "iiii" + "ff" + "ppp" + "p"),
+    "hb200_gaussian_ppo_loss_workspace_bytes": ("z", "iii"),
+    "hb200_gaussian_ppo_loss": ("i", "pppppp" + "pppppp" + "iiii" + "ff" + "fff" + "ii" + "ppp" + "pppppp" + "pp" + "p"),
     "hb200_clip_adam_workspace_bytes": ("z", "l"),
     "hb200_grad_sqnorm": ("i", "plfppp"),
     "hb200_clip_adam": ("i", "pppp" + "l" + "fffffff" + "l" + "pppp"),
@@ -98,6 +101,8 @@ SIGNATURES = {
     "hb200_sensor_linear_bwd": ("i", "pipii" + "p" + "iii" + "pp" + "p"),
     "hb200_index_embed_fwd": ("i", "pppii" + "pip" + "ii" + "p"),
     "hb200_index_embed_bwd": ("i", "pppiii" + "p" + "ii" + "p" + "p"),
+    "hb200_prev_action_linear_fwd": ("i", "ppii" + "ppp" + "ii" + "p"),
+    "hb200_prev_action_linear_bwd": ("i", "ppii" + "p" + "ii" + "pp" + "p"),
     "hb200_prep_generic": ("i", "pppp" + "i" + "p" + "iii" + "pppp" + "p"),
     "hb200_obs_resample": ("i", "ppp" + "ii" + "p"),
 }

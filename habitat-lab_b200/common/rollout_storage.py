@@ -12,15 +12,18 @@ import torch
 
 from .. import ops
 from ..rl.resnet_policy import RolloutObservations
+from . import spaces
 from .baseline_registry import baseline_registry
 from .tensor_dict import TensorDict
 
 
 def get_action_space_info(ac_space):
-    """utils/common.py get_action_space_info for the spaces the hot path supports."""
-    if hasattr(ac_space, "n"):
+    """utils/common.py get_action_space_info for the spaces the hot path supports: Discrete -> ((1,), True), a 1-D Box
+    of A dimensions -> ((A,), False); other action spaces raise NotImplementedError."""
+    dim = spaces.continuous_action_dim(ac_space)
+    if dim is None:
         return (1,), True
-    return tuple(ac_space.shape), False
+    return (dim,), False
 
 
 @baseline_registry.register_storage

@@ -52,3 +52,16 @@ class Dict(Space):
 
     def __len__(self):
         return len(self.spaces)
+
+
+def continuous_action_dim(space):
+    """Number of action dimensions of a 1-D Box action space (continuous control), None for a discrete one (any space
+    with `.n`, as before).  Any other action space (MultiDiscrete, Dict, a Box of another rank) raises
+    NotImplementedError."""
+    if hasattr(space, "n"):
+        return None
+    kind = type(space).__name__
+    if kind == "Box" and len(space.shape) == 1:
+        return int(space.shape[0])
+    raise NotImplementedError(f"action space {kind} {getattr(space, 'shape', None)}: only Discrete and 1-D Box action "
+                              "spaces are implemented")

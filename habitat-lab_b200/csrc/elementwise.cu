@@ -1202,6 +1202,41 @@ __global__ void index_embed_bwd_kernel(const int64_t* __restrict__ idx, const in
   parts[(size_t)blockIdx.y * nacc + i] = v;
 }
 
+// Continuous previous action (resnet_policy.py:755-757): nn.Linear(A, 32) of masks * prev_actions.float().  The mask is
+// a multiplication, as the reference's, so a NaN / inf previous action of a masked frame still gives NaN.
+__global__ void prev_action_linear_fwd_kernel(const float* __restrict__ pa, const uint8_t* __restrict__ masks, int B,
+                                              int A, const float* __restrict__ w, const float* __restrict__ b,
+                                              float* __restrict__ out, int ld, int col0) {
+  const long long total = (long long)B * 32;
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total;
+       i += (long long)gridDim.x * blockDim.x) {
+    const int f = (int)(i >> 5), j = (int)(i & 31);
+    const float m = masks[f] ? 1.f : 0.f;
+    float v = b[j];
+    for (int k = 0; k < A; ++k) v = fmaf(w[j * A + k], m * pa[(size_t)f * A + k], v);
+    out[(size_t)f * ld + col0 + j] = v;
+  }
+}
+// Thread i owns accumulator i of [d_w (32 x A) | d_b (32)] and walks the frames of chunk blockIdx.y in order; the
+// per-chunk partials are added in order by reduce_partials.
+__global__ void prev_action_linear_bwd_kernel(const float* __restrict__ pa, const uint8_t* __restrict__ masks, int B,
+                                              int A, const float* __restrict__ d_out, int ld, int col0,
+                                              float* __restrict__ parts) {
+  const int nacc = 32 * (A + 1);
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= nacc) return;
+  const bool bias = i >= 32 * A;
+  const int j = bias ? i - 32 * A : i / A, k = bias ? 0 : i - j * A;
+  const int f0 = blockIdx.y * kEmbedFrames, f1 = min(B, f0 + kEmbedFrames);
+  float v = 0.f;
+  for (int f = f0; f < f1; ++f) {
+    const float d = d_out[(size_t)f * ld + col0 + j];
+    if (bias) { v += d; continue; }
+    v = fmaf(d, (masks[f] ? 1.f : 0.f) * pa[(size_t)f * A + k], v);
+  }
+  parts[(size_t)blockIdx.y * nacc + i] = v;
+}
+
 // ---- generic visual input prep: any mix of u8 / f32 / i32 HWC sensors, any H x W ----------------------------------
 // (ResNetEncoder.forward, resnet_policy.py:255-271: per-key permute, u8 keys scaled by 1 / high, channel concat,
 // avg_pool2d(2) -- the odd last row / column is dropped -- then RunningMeanAndVar.)  One thread per pooled pixel;
@@ -2284,6 +2319,40 @@ extern "C" int hb200_index_embed_bwd(const int64_t* idx, const int32_t* frame_ro
   HB_LAUNCH_OK();
   count_launch(1);
   return reduce_partials(parts, nparts, nacc, nacc, d_table, parts + (size_t)nparts * nacc, st);
+}
+
+extern "C" int hb200_prev_action_linear_fwd(const float* prev_actions, const uint8_t* masks, int batch, int n_actions,
+                                            const float* w, const float* b, float* out, int ld, int col0,
+                                            hb200_stream_t stream) {
+  HB_CHECK_ARG(prev_actions && masks && w && b && out && batch > 0, "prev_action_linear_fwd: bad args");
+  HB_CHECK_ARG(n_actions >= 1 && n_actions <= 64, "prev_action_linear_fwd: n_actions=%d unsupported (1..64)", n_actions);
+  prev_action_linear_fwd_kernel<<<grid_for((long long)batch * 32, 256), 256, 0, (cudaStream_t)stream>>>(
+      prev_actions, masks, batch, n_actions, w, b, out, ld, col0);
+  HB_LAUNCH_OK();
+  count_launch(1);
+  return HB200_OK;
+}
+
+extern "C" int hb200_prev_action_linear_bwd(const float* prev_actions, const uint8_t* masks, int batch, int n_actions,
+                                            const float* d_out, int ld, int col0, float* d_w, float* d_b,
+                                            hb200_stream_t stream) {
+  HB_CHECK_ARG(prev_actions && masks && d_out && d_w && d_b && batch > 0, "prev_action_linear_bwd: bad args");
+  HB_CHECK_ARG(n_actions >= 1 && n_actions <= 64, "prev_action_linear_bwd: n_actions=%d unsupported (1..64)", n_actions);
+  const int nacc = 32 * (n_actions + 1), nparts = cdiv(batch, kEmbedFrames);
+  HB_CHECK_ARG(nparts <= 65535, "prev_action_linear_bwd: batch %d exceeds %d frames", batch, 65535 * kEmbedFrames);
+  cudaStream_t st = (cudaStream_t)stream;
+  float* parts = nullptr;
+  int* tickets = nullptr;
+  int rc = stream_workspace(st, (size_t)(nparts + kReduceChunks) * nacc, 0, &parts, &tickets);
+  if (rc) return rc;
+  float* tmp = parts + (size_t)nparts * nacc;
+  prev_action_linear_bwd_kernel<<<dim3(cdiv(nacc, 128), nparts), 128, 0, st>>>(prev_actions, masks, batch, n_actions,
+                                                                               d_out, ld, col0, parts);
+  HB_LAUNCH_OK();
+  count_launch(1);
+  rc = reduce_partials(parts, nparts, nacc, 32LL * n_actions, d_w, tmp, st);
+  if (!rc) rc = reduce_partials(parts + 32 * n_actions, nparts, nacc, 32, d_b, tmp, st);
+  return rc;
 }
 
 extern "C" int hb200_prep_generic(const void* const* h_srcs, const int* h_dtypes, const int* h_channels,

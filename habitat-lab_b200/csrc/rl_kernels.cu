@@ -571,6 +571,358 @@ extern "C" int hb200_ppo_loss(const float* features, const float* w_act, const f
 }
 
 // =====================================================================================
+// Gaussian action head: act tail + PPO loss  (HB/utils/common.py:99-175 GaussianNet / CustomNormal,
+//                                             HB/rl/ppo/policy.py:330-342, HB/rl/ppo/ppo.py:195-250)
+// =====================================================================================
+// One warp per frame.  mu_maybe_std = features @ W^T + b (A rows, plus A std rows without use_std_param) and the critic
+// are length-H dot products reduced across the warp; lane a < A then owns action dimension a: its mean, standard
+// deviation, log-probability and entropy term (and, in the loss, their gradients), and the per-frame sums over the
+// action dimensions are warp sums.  Weights are read through the read-only cache: at most (2A + 1) x H floats.
+constexpr int kMaxGaussA = 16;
+constexpr float kHalfLog2Pi = 0.91893853320467274f;     // log(sqrt(2 pi))
+constexpr float kEntConst = 1.4189385332046727f;        // 0.5 + log(sqrt(2 pi))
+
+struct GaussFrame {
+  float mu_pre, s0, s2, mu, std, v;   // lane a < A: pre-activation mean, raw std, std before softplus, mean, std; all: value
+};
+
+template <int NJ>
+__device__ __forceinline__ GaussFrame gauss_frame(const float* __restrict__ xrow, const float* __restrict__ w_mu,
+                                                  const float* __restrict__ b_mu, const float* __restrict__ std_p,
+                                                  const float* __restrict__ w_val, const float* __restrict__ b_val,
+                                                  int A, int flags, float lo, float hi, int lane) {
+  constexpr int H = NJ * 32;
+  float x[NJ];
+#pragma unroll
+  for (int j = 0; j < NJ; ++j) x[j] = xrow[lane + 32 * j];
+  const bool std_param = flags & HB200_GAUSS_STD_PARAM;
+  const int L = std_param ? A : 2 * A;
+  GaussFrame g;
+  g.mu_pre = 0.f;
+  g.s0 = (std_param && lane < A) ? __ldg(std_p + lane) : 0.f;
+  for (int o = 0; o < L; ++o) {
+    float acc = 0.f;
+#pragma unroll
+    for (int j = 0; j < NJ; ++j) acc = fmaf(x[j], __ldg(w_mu + (size_t)o * H + lane + 32 * j), acc);
+    const float z = warp_sum(acc) + __ldg(b_mu + o);
+    if (o < A) {
+      if (lane == o) g.mu_pre = z;
+    } else if (lane == o - A) {
+      g.s0 = z;
+    }
+  }
+  float acc = 0.f;
+#pragma unroll
+  for (int j = 0; j < NJ; ++j) acc = fmaf(x[j], __ldg(w_val + lane + 32 * j), acc);
+  g.v = warp_sum(acc) + __ldg(b_val);
+  // GaussianNet.forward's order: tanh(mu); clamp(std); exp (log-std); softplus (threshold 20, as F.softplus)
+  g.mu = (flags & HB200_GAUSS_TANH) ? tanhf(g.mu_pre) : g.mu_pre;
+  float s = (flags & HB200_GAUSS_CLAMP_STD) ? clamp_nan(g.s0, lo, hi) : g.s0;
+  if (flags & HB200_GAUSS_LOG_STD) s = expf(s);
+  g.s2 = s;
+  if (flags & HB200_GAUSS_SOFTPLUS) s = s > 20.f ? s : log1pf(expf(s));
+  g.std = s;
+  return g;
+}
+
+// Normal(mu, std).log_prob(x) as torch.distributions.Normal writes it
+__device__ __forceinline__ float gauss_logp(float x, float mu, float std) {
+  const float d = x - mu;
+  return -(d * d) / (2.f * (std * std)) - logf(std) - kHalfLog2Pi;
+}
+
+template <int NJ>
+__global__ void __launch_bounds__(256)
+gaussian_act_kernel(const float* __restrict__ feat, const float* __restrict__ w_mu, const float* __restrict__ b_mu,
+                    const float* __restrict__ std_p, const float* __restrict__ w_val, const float* __restrict__ b_val,
+                    const float* __restrict__ eps, int B, int A, int flags, float lo, float hi,
+                    float* __restrict__ actions, float* __restrict__ alp, float* __restrict__ values) {
+  constexpr int H = NJ * 32;
+  const int lane = threadIdx.x & 31;
+  const int f = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (f >= B) return;
+  const GaussFrame g = gauss_frame<NJ>(feat + (size_t)f * H, w_mu, b_mu, std_p, w_val, b_val, A, flags, lo, hi, lane);
+  float lp = 0.f;
+  if (lane < A) {
+    // rsample: loc + eps * scale (two roundings, as torch evaluates it); deterministic: the mean
+    const float a = eps ? __fadd_rn(g.mu, __fmul_rn(eps[(size_t)f * A + lane], g.std)) : g.mu;
+    actions[(size_t)f * A + lane] = a;
+    lp = gauss_logp(a, g.mu, g.std);
+  }
+  lp = warp_sum(lp);
+  if (lane == 0) {
+    alp[f] = lp;
+    values[f] = g.v;
+  }
+}
+
+extern "C" int hb200_gaussian_act(const float* features, const float* w_mu, const float* b_mu, const float* std_param,
+                                  const float* w_val, const float* b_val, const float* eps, int batch, int hidden,
+                                  int n_actions, int flags, float min_std, float max_std, float* actions,
+                                  float* action_log_probs, float* values, hb200_stream_t stream) {
+  HB_CHECK_ARG(features && w_mu && b_mu && w_val && b_val && actions && action_log_probs && values,
+               "gaussian_act: null pointer");
+  HB_CHECK_ARG(batch > 0 && n_actions >= 1 && n_actions <= kMaxGaussA, "gaussian_act: n_actions=%d unsupported (1..%d)",
+               n_actions, kMaxGaussA);
+  HB_CHECK_ARG(hidden == 32 || hidden == 64 || hidden == 128 || hidden == 256 || hidden == 512,
+               "gaussian_act: hidden=%d unsupported (32,64,128,256,512)", hidden);
+  HB_CHECK_ARG((flags & ~HB200_GAUSS_ALL_FLAGS) == 0, "gaussian_act: unknown flags 0x%x", flags);
+  HB_CHECK_ARG(!(flags & HB200_GAUSS_STD_PARAM) == !std_param, "gaussian_act: std_param must be given iff use_std_param");
+  cudaStream_t st = (cudaStream_t)stream;
+  const int grid = cdiv(batch, 8);
+#define HB_GACT_LAUNCH(NJ)                                                                                            \
+  gaussian_act_kernel<NJ><<<grid, 256, 0, st>>>(features, w_mu, b_mu, std_param, w_val, b_val, eps, batch, n_actions, \
+                                                flags, min_std, max_std, actions, action_log_probs, values)
+  switch (hidden) {
+    case 32: HB_GACT_LAUNCH(1); break;
+    case 64: HB_GACT_LAUNCH(2); break;
+    case 128: HB_GACT_LAUNCH(4); break;
+    case 256: HB_GACT_LAUNCH(8); break;
+    default: HB_GACT_LAUNCH(16); break;
+  }
+#undef HB_GACT_LAUNCH
+  HB_LAUNCH_OK();
+  count_launch(1);
+  return HB200_OK;
+}
+
+// dl row of a frame (C = 2A + 1 columns): [0, L) d mu_maybe_std outputs (L = A with use_std_param, else 2A), L: d value,
+// and with use_std_param [A + 1, 2A + 1): this frame's gradient of the std parameter.
+template <int NJ>
+__global__ void __launch_bounds__(256, 2)
+gaussian_loss_main_kernel(const float* __restrict__ feat, const float* __restrict__ w_mu, const float* __restrict__ b_mu,
+                          const float* __restrict__ std_p, const float* __restrict__ w_val,
+                          const float* __restrict__ b_val, const float* __restrict__ actions,
+                          const float* __restrict__ old_lp, const float* __restrict__ advs,
+                          const float* __restrict__ old_v, const float* __restrict__ rets,
+                          const float* __restrict__ is_coeffs, int B, int A, int flags, float lo, float hi, float clip,
+                          float c_v, float c_e, int use_clip_v, int compute_grads, float* __restrict__ values_o,
+                          float* __restrict__ lp_o, float* __restrict__ ent_o, float* __restrict__ d_feat,
+                          float* __restrict__ dl, LossPartial* __restrict__ partials) {
+  constexpr int H = NJ * 32;
+  __shared__ LossPartial wpart[8];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int nwarps = gridDim.x * (blockDim.x >> 5);
+  const float invB = 1.0f / (float)B;
+  const bool std_param = flags & HB200_GAUSS_STD_PARAM;
+  const int L = std_param ? A : 2 * A, C = 2 * A + 1;
+  LossPartial p = {0, 0, 0, 0, 0, 0, INFINITY, -INFINITY, INFINITY, -INFINITY, 0, 0};
+
+  for (int f = blockIdx.x * (blockDim.x >> 5) + warp; f < B; f += nwarps) {
+    const GaussFrame g = gauss_frame<NJ>(feat + (size_t)f * H, w_mu, b_mu, std_p, w_val, b_val, A, flags, lo, hi, lane);
+    const float xa = lane < A ? actions[(size_t)f * A + lane] : 0.f;
+    const float lp = warp_sum(lane < A ? gauss_logp(xa, g.mu, g.std) : 0.f);
+    const float ent = warp_sum(lane < A ? kEntConst + logf(g.std) : 0.f);
+    const float v = g.v;
+    const float adv = advs[f], ov = old_v[f], ret = rets[f];
+    const float isw = is_coeffs ? min_nan(is_coeffs[f], 1.0f) : 1.0f;
+    const float ratio = expf(lp - old_lp[f]);
+    const float s1 = adv * ratio;
+    const float s2 = adv * clamp_nan(ratio, 1.0f - clip, 1.0f + clip);
+    const float a_loss = -min_nan(s1, s2);
+    float v_used = v;
+    bool v_live = true;
+    if (use_clip_v) {
+      const float delta = v - ov;
+      v_live = fabsf(delta) < clip;
+      if (!v_live) v_used = ov + clamp_nan(delta, -clip, clip);
+    }
+    const float dv = v_used - ret;
+    const float v_loss = 0.5f * dv * dv;
+
+    if (lane == 0) {
+      if (values_o) values_o[f] = v;
+      if (lp_o) lp_o[f] = lp;
+      if (ent_o) ent_o[f] = ent;
+      p.vl += isw * v_loss; p.al += isw * a_loss; p.ent += isw * ent;
+      p.vsum += v; p.rsum += ratio;
+      p.nclip += (ratio > 1.0f + clip ? 1.f : 0.f) + (ratio < 1.0f - clip ? 1.f : 0.f);
+      p.vmin = min_nan(p.vmin, v); p.vmax = max_nan(p.vmax, v);
+      p.rmin = min_nan(p.rmin, ratio); p.rmax = max_nan(p.rmax, ratio);
+    }
+    if (compute_grads) {
+      // as in ppo_loss_main_kernel: d total / d lp, d value, d entropy (each already / B)
+      const float g_lp = !(s1 > s2) ? (-adv * ratio) * isw * invB : 0.f;
+      const float g_v = v_live ? c_v * dv * isw * invB : 0.f;
+      const float g_h = -c_e * isw * invB;
+      float dmu_pre = 0.f, ds0 = 0.f;
+      if (lane < A) {
+        const float d = xa - g.mu, sd = g.std, var = sd * sd;
+        const float dmu = g_lp * (d / var);
+        // d log_prob / d std = d^2 / std^3 - 1 / std;  d entropy / d std = 1 / std
+        float ds = g_lp * ((d * d) / (var * sd) - 1.f / sd) + g_h / sd;
+        dmu_pre = (flags & HB200_GAUSS_TANH) ? dmu * (1.f - g.mu * g.mu) : dmu;
+        if (flags & HB200_GAUSS_SOFTPLUS) {
+          if (!(g.s2 > 20.f)) {
+            const float z = expf(g.s2);
+            ds = ds * z / (z + 1.f);
+          }
+        }
+        if (flags & HB200_GAUSS_LOG_STD) ds = ds * g.s2;
+        // clamp's backward passes the gradient where lo <= x <= hi (bounds included) and gives 0 elsewhere (NaN too)
+        if ((flags & HB200_GAUSS_CLAMP_STD) && !(g.s0 >= lo && g.s0 <= hi)) ds = 0.f;
+        ds0 = ds;
+        float* row = dl + (size_t)f * C;
+        row[lane] = dmu_pre;
+        row[std_param ? A + 1 + lane : A + lane] = ds0;
+      }
+      if (lane == 0) dl[(size_t)f * C + L] = g_v;
+      // d_features = sum_o dl_o W_o + g_v w_val, in row order
+      float acc[NJ];
+#pragma unroll
+      for (int j = 0; j < NJ; ++j) acc[j] = 0.f;
+      for (int o = 0; o < L; ++o) {
+        const float dz = o < A ? __shfl_sync(0xffffffffu, dmu_pre, o) : __shfl_sync(0xffffffffu, ds0, o - A);
+#pragma unroll
+        for (int j = 0; j < NJ; ++j) acc[j] = fmaf(dz, __ldg(w_mu + (size_t)o * H + lane + 32 * j), acc[j]);
+      }
+#pragma unroll
+      for (int j = 0; j < NJ; ++j) d_feat[(size_t)f * H + lane + 32 * j] = fmaf(g_v, __ldg(w_val + lane + 32 * j), acc[j]);
+    }
+  }
+  if (lane == 0) wpart[warp] = p;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    LossPartial r = wpart[0];
+    for (int w = 1; w < (int)(blockDim.x >> 5); ++w) {
+      const LossPartial q = wpart[w];
+      r.vl += q.vl; r.al += q.al; r.ent += q.ent; r.vsum += q.vsum; r.rsum += q.rsum; r.nclip += q.nclip;
+      r.vmin = min_nan(r.vmin, q.vmin); r.vmax = max_nan(r.vmax, q.vmax);
+      r.rmin = min_nan(r.rmin, q.rmin); r.rmax = max_nan(r.rmax, q.rmax);
+    }
+    partials[blockIdx.x] = r;
+  }
+}
+
+// Weight rows R = L + 1 (mu_maybe_std rows, then the critic): parts[y] = [dW (R x H) | column sums of dl (C = 2A + 1)]
+// for frame slab y = blockIdx.y, summed over slabs in order by reduce_partials (no floating-point atomics).
+constexpr int kMaxGaussRows = 2 * kMaxGaussA + 1;
+__global__ void __launch_bounds__(256, 2)
+gaussian_heads_wgrad_kernel(const float* __restrict__ feat, const float* __restrict__ dl, int B, int H, int R, int C,
+                            float* __restrict__ parts) {
+  float* prow = parts + (size_t)blockIdx.y * ((size_t)R * H + C);
+  __shared__ float red[8][kMaxGaussRows][32];
+  __shared__ float bred[8][64];
+  const int lane = threadIdx.x & 31;
+  const int col = blockIdx.x * 32 + lane;
+  const int slice = threadIdx.x >> 5;
+  const int per = (B + gridDim.y - 1) / gridDim.y;
+  const int b0 = blockIdx.y * per, b1 = min(B, b0 + per);
+  float acc[kMaxGaussRows];
+#pragma unroll
+  for (int r = 0; r < kMaxGaussRows; ++r) acc[r] = 0.f;
+  float bacc0 = 0.f, bacc1 = 0.f;   // column sums of dl: columns lane and lane + 32 (block column 0 only)
+  for (int b = b0 + slice; b < b1; b += 8) {
+    const float x = (col < H) ? feat[(size_t)b * H + col] : 0.f;
+    const float* drow = dl + (size_t)b * C;
+#pragma unroll
+    for (int r = 0; r < kMaxGaussRows; ++r)
+      if (r < R) acc[r] = fmaf(drow[r], x, acc[r]);
+    if (blockIdx.x == 0) {
+      if (lane < C) bacc0 += drow[lane];
+      if (lane + 32 < C) bacc1 += drow[lane + 32];
+    }
+  }
+#pragma unroll
+  for (int r = 0; r < kMaxGaussRows; ++r)
+    if (r < R) red[slice][r][lane] = acc[r];
+  bred[slice][lane] = bacc0;
+  bred[slice][lane + 32] = bacc1;
+  __syncthreads();
+  if (slice == 0 && col < H) {
+    for (int r = 0; r < R; ++r) {
+      float s = 0.f;
+      for (int w = 0; w < 8; ++w) s += red[w][r][lane];
+      prow[(size_t)r * H + col] = s;
+    }
+  }
+  if (blockIdx.x == 0 && slice < 2) {
+    const int c = lane + 32 * slice;
+    if (c < C) {
+      float s = 0.f;
+      for (int w = 0; w < 8; ++w) s += bred[w][c];
+      prow[(size_t)R * H + c] = s;
+    }
+  }
+}
+
+extern "C" size_t hb200_gaussian_ppo_loss_workspace_bytes(int batch, int hidden, int n_actions) {
+  (void)hidden;
+  return sizeof(LossPartial) * (size_t)(kNumSMs * 2) + 256 + sizeof(float) * (size_t)batch * (2 * n_actions + 1);
+}
+
+extern "C" int hb200_gaussian_ppo_loss(const float* features, const float* w_mu, const float* b_mu,
+                                       const float* std_param, const float* w_val, const float* b_val,
+                                       const float* actions, const float* old_log_probs, const float* advantages,
+                                       const float* old_values, const float* returns, const float* is_coeffs,
+                                       int batch, int hidden, int n_actions, int flags, float min_std, float max_std,
+                                       float clip_param, float value_loss_coef, float entropy_coef,
+                                       int use_clipped_value_loss, int compute_grads, float* values, float* log_probs,
+                                       float* entropy, float* d_features, float* d_w_mu, float* d_b_mu, float* d_std,
+                                       float* d_w_val, float* d_b_val, float* metrics, void* workspace,
+                                       hb200_stream_t stream) {
+  HB_CHECK_ARG(features && w_mu && b_mu && w_val && b_val && actions && old_log_probs && advantages && old_values &&
+                   returns && metrics && workspace,
+               "gaussian_ppo_loss: null pointer");
+  HB_CHECK_ARG(batch > 0 && n_actions >= 1 && n_actions <= kMaxGaussA,
+               "gaussian_ppo_loss: n_actions=%d unsupported (1..%d)", n_actions, kMaxGaussA);
+  HB_CHECK_ARG(hidden == 32 || hidden == 64 || hidden == 128 || hidden == 256 || hidden == 512,
+               "gaussian_ppo_loss: hidden=%d unsupported (32,64,128,256,512)", hidden);
+  HB_CHECK_ARG((flags & ~HB200_GAUSS_ALL_FLAGS) == 0, "gaussian_ppo_loss: unknown flags 0x%x", flags);
+  const bool sp = flags & HB200_GAUSS_STD_PARAM;
+  HB_CHECK_ARG(!sp == !std_param, "gaussian_ppo_loss: std_param must be given iff use_std_param");
+  HB_CHECK_ARG(!compute_grads || (d_features && d_w_mu && d_b_mu && d_w_val && d_b_val && (!sp || d_std)),
+               "gaussian_ppo_loss: compute_grads needs gradient outputs");
+  cudaStream_t st = (cudaStream_t)stream;
+  LossPartial* partials = (LossPartial*)workspace;
+  float* dl = (float*)((char*)workspace + ((sizeof(LossPartial) * (size_t)(kNumSMs * 2) + 255) / 256) * 256);
+  const int grid = loss_grid(batch);
+#define HB_GLOSS_LAUNCH(NJ)                                                                                        \
+  gaussian_loss_main_kernel<NJ><<<grid, 256, 0, st>>>(                                                             \
+      features, w_mu, b_mu, std_param, w_val, b_val, actions, old_log_probs, advantages, old_values, returns,      \
+      is_coeffs, batch, n_actions, flags, min_std, max_std, clip_param, value_loss_coef, entropy_coef,             \
+      use_clipped_value_loss, compute_grads, values, log_probs, entropy, d_features, dl, partials)
+  switch (hidden) {
+    case 32: HB_GLOSS_LAUNCH(1); break;
+    case 64: HB_GLOSS_LAUNCH(2); break;
+    case 128: HB_GLOSS_LAUNCH(4); break;
+    case 256: HB_GLOSS_LAUNCH(8); break;
+    default: HB_GLOSS_LAUNCH(16); break;
+  }
+#undef HB_GLOSS_LAUNCH
+  HB_LAUNCH_OK();
+  ppo_loss_finalize_kernel<<<1, 32, 0, st>>>(partials, grid, batch, value_loss_coef, entropy_coef, metrics);
+  HB_LAUNCH_OK();
+  count_launch(2);
+  if (compute_grads) {
+    const int A = n_actions, L = sp ? A : 2 * A, R = L + 1, C = 2 * A + 1;
+    const long long H = hidden;
+    HB_CUDA(cudaMemsetAsync(d_w_mu, 0, sizeof(float) * (size_t)L * H, st));
+    HB_CUDA(cudaMemsetAsync(d_b_mu, 0, sizeof(float) * L, st));
+    HB_CUDA(cudaMemsetAsync(d_w_val, 0, sizeof(float) * H, st));
+    HB_CUDA(cudaMemsetAsync(d_b_val, 0, sizeof(float), st));
+    if (sp) HB_CUDA(cudaMemsetAsync(d_std, 0, sizeof(float) * A, st));
+    dim3 g(cdiv(hidden, 32), min(32, cdiv(batch, 64)));
+    const long long row = (long long)R * H + C;   // one partial row per frame slab
+    float* parts = nullptr;
+    int* tickets = nullptr;
+    int rc = stream_workspace(st, (size_t)(g.y + kReduceChunks) * row, 0, &parts, &tickets);
+    if (rc) return rc;
+    float* tmp = parts + (size_t)g.y * row;
+    gaussian_heads_wgrad_kernel<<<g, 256, 0, st>>>(features, dl, batch, hidden, R, C, parts);
+    HB_LAUNCH_OK();
+    count_launch(1);
+    rc = reduce_partials(parts, g.y, row, (long long)L * H, d_w_mu, tmp, st);
+    if (!rc) rc = reduce_partials(parts + (size_t)L * H, g.y, row, H, d_w_val, tmp, st);
+    if (!rc) rc = reduce_partials(parts + (size_t)R * H, g.y, row, L, d_b_mu, tmp, st);
+    if (!rc) rc = reduce_partials(parts + (size_t)R * H + L, g.y, row, 1, d_b_val, tmp, st);
+    if (!rc && sp) rc = reduce_partials(parts + (size_t)R * H + A + 1, g.y, row, A, d_std, tmp, st);
+    if (rc) return rc;
+  }
+  return HB200_OK;
+}
+
+// =====================================================================================
 // clip_grad_norm_ + Adam  (HB/rl/ppo/ppo.py:112-137,257,347-371; torch.optim.Adam math)
 // =====================================================================================
 __global__ void sqnorm_partial_kernel(const float* __restrict__ g, long long n, float scale,

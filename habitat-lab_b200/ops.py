@@ -69,6 +69,44 @@ def ppo_loss(features, w_act, b_act, w_val, b_val, actions, old_lp, adv, old_v, 
          ptr(out.get("d_w_val")), ptr(out.get("d_b_val")), ptr(out["metrics"]), ptr(workspace))
 
 
+# ---- Gaussian action head --------------------------------------------------------------------------
+GAUSS_LOG_STD, GAUSS_SOFTPLUS, GAUSS_STD_PARAM, GAUSS_CLAMP_STD, GAUSS_TANH = 1, 2, 4, 8, 16
+
+
+def gaussian_act(features, w_mu, b_mu, std_param, w_val, b_val, eps, flags, min_std, max_std, actions,
+                 action_log_probs, values):
+    """eps: f32 [B, A] standard-normal draws (actions = mu + eps * std), or None for the mean."""
+    B, H = features.shape
+    A = actions.shape[-1]
+    _chk(features, torch.float32, "features")
+    _chk(actions, torch.float32, "actions")
+    if eps is not None:
+        _chk(eps, torch.float32, "eps")
+    call("hb200_gaussian_act", ptr(features), ptr(w_mu), ptr(b_mu), ptr(std_param), ptr(w_val), ptr(b_val), ptr(eps),
+         B, H, A, int(flags), float(min_std), float(max_std), ptr(actions), ptr(action_log_probs), ptr(values))
+
+
+def gaussian_ppo_loss_workspace(batch, hidden, n_actions, device):
+    nbytes = load().hb200_gaussian_ppo_loss_workspace_bytes(batch, hidden, n_actions)
+    return torch.empty(nbytes, dtype=torch.uint8, device=device)
+
+
+def gaussian_ppo_loss(features, w_mu, b_mu, std_param, w_val, b_val, actions, old_lp, adv, old_v, returns, flags,
+                      min_std, max_std, clip, c_v, c_e, use_clipped_value_loss, compute_grads, out, workspace,
+                      is_coeffs=None):
+    """actions f32 [B, A]; out: like ppo_loss's, with d_w_mu / d_b_mu / d_std for the action head."""
+    B, H = features.shape
+    A = actions.shape[-1]
+    _chk(features, torch.float32, "features")
+    _chk(actions, torch.float32, "actions")
+    call("hb200_gaussian_ppo_loss", ptr(features), ptr(w_mu), ptr(b_mu), ptr(std_param), ptr(w_val), ptr(b_val),
+         ptr(actions), ptr(old_lp), ptr(adv), ptr(old_v), ptr(returns), ptr(is_coeffs), B, H, A, int(flags),
+         float(min_std), float(max_std), float(clip), float(c_v), float(c_e), int(bool(use_clipped_value_loss)),
+         int(bool(compute_grads)), ptr(out.get("values")), ptr(out.get("log_probs")), ptr(out.get("entropy")),
+         ptr(out.get("d_features")), ptr(out.get("d_w_mu")), ptr(out.get("d_b_mu")), ptr(out.get("d_std")),
+         ptr(out.get("d_w_val")), ptr(out.get("d_b_val")), ptr(out["metrics"]), ptr(workspace))
+
+
 # ---- optimizer ----------------------------------------------------------------------------------
 def clip_adam_workspace(n, device):
     return torch.empty(load().hb200_clip_adam_workspace_bytes(n), dtype=torch.uint8, device=device)
@@ -488,6 +526,20 @@ def index_embed_fwd(idx, frame_rows, masks, table, out, col0, batch):
 def index_embed_bwd(idx, frame_rows, masks, d_out, col0, d_table, batch):
     call("hb200_index_embed_bwd", ptr(idx), ptr(frame_rows), ptr(as_u8(masks) if masks is not None else None), int(batch),
          d_table.shape[0], d_table.shape[1], ptr(d_out), d_out.stride(0), int(col0), ptr(d_table))
+
+
+def prev_action_linear_fwd(prev_actions, masks, w, b, out, col0):
+    """continuous previous action: out[:, col0:col0+32] = Linear(A, 32)(masks * prev_actions), prev_actions f32 [B, A]"""
+    _chk(prev_actions, torch.float32, "prev_actions")
+    B, A = prev_actions.shape
+    call("hb200_prev_action_linear_fwd", ptr(prev_actions), ptr(as_u8(masks)), B, A, ptr(w), ptr(b), ptr(out),
+         out.stride(0), int(col0))
+
+
+def prev_action_linear_bwd(prev_actions, masks, d_out, col0, d_w, d_b):
+    B, A = prev_actions.shape
+    call("hb200_prev_action_linear_bwd", ptr(prev_actions), ptr(as_u8(masks)), B, A, ptr(d_out), d_out.stride(0),
+         int(col0), ptr(d_w), ptr(d_b))
 
 
 _PREP_DTYPE = {torch.uint8: 0, torch.float32: 1, torch.int32: 2}

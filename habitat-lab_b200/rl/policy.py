@@ -79,7 +79,11 @@ class PointNavBaselineNet(nn.Module):
 
 @baseline_registry.register_policy
 class PointNavBaselinePolicy(NativeNetPolicy):
-    def __init__(self, observation_space, action_space, hidden_size: int = 512, aux_loss_config=None, **kwargs):
+    def __init__(self, observation_space, action_space, hidden_size: int = 512, aux_loss_config=None,
+                 policy_config=None, **kwargs):
+        if getattr(policy_config, "action_distribution_type", "categorical") != "categorical":
+            raise NotImplementedError("PointNavBaselinePolicy (SimpleCNN) implements the categorical action "
+                                      "distribution only")
         super().__init__(PointNavBaselineNet(observation_space, hidden_size), action_space)
         self.observation_space = observation_space
         self._ws = {}
@@ -87,8 +91,15 @@ class PointNavBaselinePolicy(NativeNetPolicy):
 
     @classmethod
     def from_config(cls, config, observation_space, action_space, **kwargs):
-        return cls(observation_space=observation_space, action_space=action_space,
-                   hidden_size=config.habitat_baselines.rl.ppo.hidden_size)
+        hb = config.habitat_baselines
+        agent_name = kwargs.get("agent_name")
+        if agent_name is None:   # configs without a simulator section describe a single, categorical agent
+            simulator = getattr(getattr(config, "habitat", None), "simulator", None)
+            agent_name = getattr(simulator, "agents_order", [None])[0]
+        policies = getattr(hb.rl, "policy", {})
+        policy_cfg = policies[agent_name] if agent_name in policies else None
+        return cls(observation_space=observation_space, action_space=action_space, hidden_size=hb.rl.ppo.hidden_size,
+                   policy_config=policy_cfg)
 
     # ---- conv stack bookkeeping ------------------------------------------------------------------------
     def _layers(self):

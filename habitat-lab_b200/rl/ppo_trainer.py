@@ -19,6 +19,7 @@ from typing import Dict, Optional
 import numpy as np
 import torch
 
+from ..common import spaces
 from ..common.baseline_registry import baseline_registry
 from ..common.obs_transformers import ObsTransformPlan, apply_obs_transforms_obs_space, get_active_obs_transforms
 from ..common.rollout_storage import RolloutStorage
@@ -28,7 +29,7 @@ import os
 
 from .ppo import DDPPO, PPO  # noqa: F401  (registers the updaters)
 from . import policy as _policy  # noqa: F401  (registers PointNavBaselinePolicy)
-from .resnet_policy import VISUAL_FEATURES_KEY, PointNavResNetPolicy  # noqa: F401
+from .resnet_policy import VISUAL_FEATURES_KEY, ActionDistributionConfig, PointNavResNetPolicy  # noqa: F401
 from .single_agent_access_mgr import SingleAgentAccessMgr
 
 
@@ -74,13 +75,19 @@ class DDPPOConfig:
 
 
 def make_config(num_environments=4, total_num_steps=-1.0, num_updates=2, height=256, width=256, seed=100,
-                obs_transforms=None, ddppo=None, **ppo_kw):
+                obs_transforms=None, ddppo=None, continuous_actions=0, action_dist=None, **ppo_kw):
     """A habitat_baselines-shaped config for the synthetic PointNav DD-PPO run (ddppo_pointnav.yaml values).
     obs_transforms: {name: config node with `type` and the transformer's fields} (e.g. the ObjectNav YAMLs'
     resize_shortest_edge + center_cropper, common/obs_transformers.py); height / width are then the raw sensor size.
-    ddppo: DDPPOConfig field overrides, e.g. dict(pretrained=True, pretrained_weights=path, train_encoder=False)."""
+    ddppo: DDPPOConfig field overrides, e.g. dict(pretrained=True, pretrained_weights=path, train_encoder=False).
+    continuous_actions = A > 0: continuous control -- a Box(-1, 1, (A,)) action space and the gaussian policy
+    (monolithic.yaml), with action_dist the ActionDistributionConfig field overrides (e.g. social_nav.yaml's
+    dict(use_std_param=True))."""
     ppo = PPOConfig(**{**dict(ppo_epoch=2, num_mini_batch=2, num_steps=128, max_grad_norm=0.2), **ppo_kw})
     agent = SimpleNamespace(name="PointNavResNetPolicy", action_distribution_type="categorical")
+    if continuous_actions:
+        agent.action_distribution_type = "gaussian"
+        agent.action_dist = ActionDistributionConfig(**(action_dist or {}))
     if obs_transforms is not None:
         agent.obs_transforms = dict(obs_transforms)
     hb = SimpleNamespace(
@@ -92,7 +99,8 @@ def make_config(num_environments=4, total_num_steps=-1.0, num_updates=2, height=
         eval=SimpleNamespace(extra_sim_sensors={}),
     )
     habitat = SimpleNamespace(seed=seed, simulator=SimpleNamespace(agents_order=["main_agent"]),
-                              synthetic=SimpleNamespace(height=height, width=width, p_done=1.0 / 250.0))
+                              synthetic=SimpleNamespace(height=height, width=width, p_done=1.0 / 250.0,
+                                                        continuous_actions=int(continuous_actions)))
     return SimpleNamespace(habitat_baselines=hb, habitat=habitat)
 
 
@@ -169,6 +177,8 @@ class SyntheticVectorEnvFactory:
                        is_first_rank=True, device=None, rank=0):
         syn = config.habitat.synthetic
         obs_space, act_space = pointnav_spaces(syn.height, syn.width)
+        if getattr(syn, "continuous_actions", 0):   # the environment draws no random numbers for its actions
+            act_space = spaces.Box(-1.0, 1.0, (syn.continuous_actions,), np.float32)
         n = config.habitat_baselines.num_environments
         return SyntheticVectorEnv(n, obs_space, act_space, device, config.habitat.seed + rank * n, syn.p_done)
 
@@ -232,6 +242,10 @@ class PPOTrainer:
         self._env_spec = SimpleNamespace(observation_space=obs_space, action_space=act_space,
                                          orig_action_space=self.envs.orig_action_spaces[0])
         self._create_obs_transforms()
+        self._action_bounds = None
+        if spaces.continuous_action_dim(act_space) is not None:
+            self._action_bounds = tuple(torch.as_tensor(b, dtype=torch.float32, device=self.device)
+                                        for b in (act_space.low, act_space.high))
         self._agent = self._create_agent(None)
         if torch.distributed.is_initialized():
             self._agent.init_distributed(find_unused_params=False)
@@ -335,7 +349,10 @@ class PPOTrainer:
         ad = self.actor_critic.act(step["observations"], step["recurrent_hidden_states"], step["prev_actions"],
                                    step["masks"])
         self.timings["act"] += time.perf_counter() - t0
-        obs, rewards, dones, _ = self.envs.step(ad.actions)
+        env_actions = ad.env_actions
+        if self._action_bounds is not None:   # ppo_trainer.py:379-385: the env gets the clipped action, storage not
+            env_actions = torch.clamp(env_actions, *self._action_bounds)
+        obs, rewards, dones, _ = self.envs.step(env_actions)
         not_done = (~dones).view(-1, 1)
         self.current_episode_reward += rewards
         self.running_episode_stats["reward"] += torch.where(not_done, torch.zeros_like(rewards), self.current_episode_reward)

@@ -18,7 +18,7 @@ from __future__ import annotations
 import math
 import os
 from collections import OrderedDict
-from dataclasses import dataclass
+from dataclasses import dataclass, fields
 from typing import Dict, List, Optional
 
 import numpy as np
@@ -141,10 +141,15 @@ class PointNavResNetNet(nn.Module):
     def __init__(self, observation_space, action_space, hidden_size, num_recurrent_layers, rnn_type, backbone,
                  resnet_baseplanes, normalize_visual_inputs, fuse_keys=None, discrete_actions=True):
         super().__init__()
-        if not discrete_actions:
-            raise NotImplementedError("continuous prev-action input (gaussian policies) is a 'next' row (SURVEY 8f-4)")
         sp = observation_space.spaces
-        self.prev_action_embedding = nn.Embedding(action_space.n + 1, 32)
+        self.discrete_actions = discrete_actions
+        if discrete_actions:
+            self.prev_action_embedding = nn.Embedding(action_space.n + 1, 32)
+        else:   # resnet_policy.py:420-428: Linear(A, 32) of masks * prev_actions
+            dim = spaces.continuous_action_dim(action_space)
+            if dim is None:
+                raise NotImplementedError("a continuous previous-action input needs a 1-D Box action space")
+            self.prev_action_embedding = nn.Linear(dim, 32)
         if fuse_keys is None:
             fuse_keys = [k for k in sp.keys() if k not in _GOAL_SENSOR_KEYS]
         self._fuse_keys_1d = [k for k in fuse_keys if len(sp[k].shape) == 1]
@@ -246,6 +251,61 @@ class CategoricalNet(nn.Module):
         self.linear = nn.Linear(num_inputs, num_outputs)
         nn.init.orthogonal_(self.linear.weight, gain=0.01)
         nn.init.constant_(self.linear.bias, 0)
+
+
+@dataclass
+class ActionDistributionConfig:
+    """habitat_baselines' ActionDistributionConfig (config/default_structured_configs.py:69-86): the fields GaussianNet
+    reads, with the reference's defaults."""
+    use_log_std: bool = True
+    use_softplus: bool = False
+    log_std_init: float = 0.0
+    use_std_param: bool = False
+    clamp_std: bool = True
+    min_std: float = 1e-6
+    max_std: float = 1
+    min_log_std: float = -5
+    max_log_std: float = 2
+    action_activation: str = "tanh"
+
+
+class GaussianNet(nn.Module):
+    """Parameter holder of the reference's GaussianNet (utils/common.py:112-175): same parameters, names, initialisation
+    and random-number order; `flags`, `min_std` and `max_std` are what the Gaussian kernels take.  Fields missing from
+    `config` take ActionDistributionConfig's defaults."""
+
+    def __init__(self, num_inputs: int, num_outputs: int, config=None):
+        super().__init__()
+        cfg = {f.name: getattr(config, f.name, f.default) for f in fields(ActionDistributionConfig)}
+        self.action_activation = cfg["action_activation"]
+        self.use_softplus = bool(cfg["use_softplus"])
+        self.use_log_std = bool(cfg["use_log_std"])
+        self.clamp_std = bool(cfg["clamp_std"])
+        use_std_param = bool(cfg["use_std_param"])
+        if self.use_log_std:
+            self.min_std, self.max_std = cfg["min_log_std"], cfg["max_log_std"]
+            std_init = cfg["log_std_init"]
+        elif self.use_softplus:
+            inv_softplus = lambda x: math.log(math.exp(x) - 1)  # noqa: E731
+            self.min_std, self.max_std = inv_softplus(cfg["min_std"]), inv_softplus(cfg["max_std"])
+            std_init = inv_softplus(1.0)
+        else:
+            self.min_std, self.max_std = cfg["min_std"], cfg["max_std"]
+            std_init = 1.0
+        if use_std_param:
+            self.std = nn.Parameter(torch.randn(num_outputs) * 0.01 + std_init)
+            num_linear_outputs = num_outputs
+        else:
+            self.std = None
+            num_linear_outputs = 2 * num_outputs
+        self.mu_maybe_std = nn.Linear(num_inputs, num_linear_outputs)
+        nn.init.orthogonal_(self.mu_maybe_std.weight, gain=0.01)
+        nn.init.constant_(self.mu_maybe_std.bias, 0)
+        if not use_std_param:
+            nn.init.constant_(self.mu_maybe_std.bias[num_outputs:], std_init)
+        self.flags = ((ops.GAUSS_LOG_STD if self.use_log_std else 0) | (ops.GAUSS_SOFTPLUS if self.use_softplus else 0) |
+                      (ops.GAUSS_STD_PARAM if use_std_param else 0) | (ops.GAUSS_CLAMP_STD if self.clamp_std else 0) |
+                      (ops.GAUSS_TANH if self.action_activation == "tanh" else 0))
 
 
 class CriticHead(nn.Module):
@@ -767,13 +827,25 @@ class NativeNetPolicy(nn.Module):
       _visual_backward(d_rnn_in f32 [B, D], saved, B, dev)   (writes parameter gradients in place)
     """
 
-    def __init__(self, net: nn.Module, action_space):
+    def __init__(self, net: nn.Module, action_space, action_distribution_type: str = "categorical", action_dist=None):
         super().__init__()
-        self.action_distribution_type = "categorical"
+        continuous_dim = spaces.continuous_action_dim(action_space)
+        if action_distribution_type not in ("categorical", "gaussian"):
+            raise NotImplementedError(f"action_distribution_type {action_distribution_type!r}: categorical and gaussian "
+                                      "are implemented")
+        if (action_distribution_type == "gaussian") != (continuous_dim is not None):
+            raise NotImplementedError(f"a {action_distribution_type} action distribution over a "
+                                      f"{type(action_space).__name__} action space is not implemented")
+        self.action_distribution_type = action_distribution_type
+        self._gaussian = action_distribution_type == "gaussian"
         self._action_space = action_space
         self.net = net
-        self.dim_actions = action_space.n
-        self.action_distribution = CategoricalNet(self.net.output_size, self.dim_actions)
+        if self._gaussian:
+            self.dim_actions = continuous_dim
+            self.action_distribution = GaussianNet(self.net.output_size, self.dim_actions, action_dist)
+        else:
+            self.dim_actions = action_space.n
+            self.action_distribution = CategoricalNet(self.net.output_size, self.dim_actions)
         self.critic = CriticHead(self.net.output_size)
         self.aux_loss_modules = nn.ModuleDict()
         self._flat = None
@@ -905,7 +977,8 @@ class NativeNetPolicy(nn.Module):
     def _loss_ws(self, B, dev):
         key = ("loss_ws", B)
         if key not in self._buf or self._buf[key].device != dev:
-            self._buf[key] = ops.ppo_loss_workspace(B, self.net.output_size, self.dim_actions, dev)
+            make = ops.gaussian_ppo_loss_workspace if self._gaussian else ops.ppo_loss_workspace
+            self._buf[key] = make(B, self.net.output_size, self.dim_actions, dev)
         return self._buf[key]
 
     # ---- recurrent state encoder -----------------------------------------------------------------------
@@ -1104,7 +1177,7 @@ class NativeNetPolicy(nn.Module):
         n = rnn_hidden_states.shape[0]
         T = B // n
         assert T * n == B, "frames must be (t, env)-ordered with T*n rows"
-        pa = prev_actions.reshape(-1)
+        pa = prev_actions.reshape(B, -1).contiguous() if self._gaussian else prev_actions.reshape(-1)
         mk = ops.as_u8(masks.reshape(-1))
         rnn_in, vsaved = self._visual_forward(obs, rows, pa, mk, B, dev, train)
         hid = rnn_hidden_states.contiguous()
@@ -1113,11 +1186,32 @@ class NativeNetPolicy(nn.Module):
                     hidden_out=hidden_out, visual=vsaved)
 
     def _heads(self, feats, B, dev):
-        logits = self._tmp("logits", (B, self.dim_actions), dev)
         values = self._tmp("values_act", (B,), dev)
-        ad, cr = self.action_distribution.linear, self.critic.fc
+        cr = self.critic.fc
+        if self._gaussian:   # the mean action and its log-probability are by-products here
+            self._gaussian_act(feats, None, self._tmp("gauss_mean", (B, self.dim_actions), dev),
+                               self._tmp("gauss_mean_lp", (B,), dev), values)
+            return None, values
+        logits = self._tmp("logits", (B, self.dim_actions), dev)
+        ad = self.action_distribution.linear
         ops.heads_fwd(feats, ad.weight, ad.bias, cr.weight, cr.bias, logits, values)
         return logits, values
+
+    def _gaussian_act(self, feats, eps, action, alp, values):
+        gn, cr = self.action_distribution, self.critic.fc
+        ops.gaussian_act(feats, gn.mu_maybe_std.weight, gn.mu_maybe_std.bias, gn.std, cr.weight, cr.bias, eps, gn.flags,
+                         gn.min_std, gn.max_std, action, alp, values)
+
+    def _gaussian_loss(self, feats, actions, old_lp, adv, old_v, ret, clip, c_v, c_e, use_clipped_value_loss,
+                       compute_grads, out, B, dev, is_coeffs=None):
+        gn, cr = self.action_distribution, self.critic.fc
+        if compute_grads:
+            out.update(d_w_mu=gn.mu_maybe_std.weight.grad, d_b_mu=gn.mu_maybe_std.bias.grad,
+                       d_std=gn.std.grad if gn.std is not None else None)
+        ops.gaussian_ppo_loss(feats, gn.mu_maybe_std.weight, gn.mu_maybe_std.bias, gn.std, cr.weight, cr.bias,
+                              actions.reshape(B, self.dim_actions).float().contiguous(), old_lp, adv, old_v, ret,
+                              gn.flags, gn.min_std, gn.max_std, clip, c_v, c_e, use_clipped_value_loss, compute_grads,
+                              out, self._loss_ws(B, dev), is_coeffs=is_coeffs)
 
     @torch.no_grad()
     def act(self, observations, rnn_hidden_states, prev_actions, masks, deterministic=False):
@@ -1128,6 +1222,14 @@ class NativeNetPolicy(nn.Module):
         B = s["B"]
         feats = s["features"]
         dev = feats.device
+        if self._gaussian:   # CustomNormal: rsample = mu + eps * std with eps from torch.randn, or the mean
+            action = torch.empty(B, self.dim_actions, dtype=torch.float32, device=dev)
+            alp = torch.empty(B, 1, dtype=torch.float32, device=dev)
+            vout = torch.empty(B, 1, dtype=torch.float32, device=dev)
+            eps = None if deterministic else torch.randn(B, self.dim_actions, device=dev, dtype=torch.float32)
+            self._gaussian_act(feats, eps, action, alp, vout)
+            return PolicyActionData(values=vout, actions=action, action_log_probs=alp,
+                                    rnn_hidden_states=s["hidden_out"])
         logp = self._tmp("logits", (B, self.dim_actions), dev)
         action = torch.empty(B, 1, dtype=torch.int64, device=dev)
         alp = torch.empty(B, 1, dtype=torch.float32, device=dev)
@@ -1153,11 +1255,14 @@ class NativeNetPolicy(nn.Module):
         dev = feats.device
         out = dict(values=self._tmp("ea_values", (B,), dev), log_probs=self._tmp("ea_lp", (B,), dev),
                    entropy=self._tmp("ea_ent", (B,), dev), metrics=self._tmp("ea_metrics", (ops.N_METRICS,), dev))
-        ad, cr = self.action_distribution.linear, self.critic.fc
         zero = self._tmp("zeros_B", (B,), dev)
         zero.zero_()
-        ops.ppo_loss(feats, ad.weight, ad.bias, cr.weight, cr.bias, action.reshape(-1), zero, zero, zero, zero, 0.2,
-                     0.5, 0.0, False, False, out, self._loss_ws(B, dev))
+        if self._gaussian:
+            self._gaussian_loss(feats, action, zero, zero, zero, zero, 0.2, 0.5, 0.0, False, False, out, B, dev)
+        else:
+            ad, cr = self.action_distribution.linear, self.critic.fc
+            ops.ppo_loss(feats, ad.weight, ad.bias, cr.weight, cr.bias, action.reshape(-1), zero, zero, zero, zero, 0.2,
+                         0.5, 0.0, False, False, out, self._loss_ws(B, dev))
         return (out["values"].view(B, 1), out["log_probs"].view(B, 1), out["entropy"].view(B, 1),
                 s["hidden_out"], {})
 
@@ -1172,16 +1277,23 @@ class NativeNetPolicy(nn.Module):
         dev = feats.device
         H = self.net.output_size
         self._flat["grads"].zero_()
-        ad, cr = self.action_distribution.linear, self.critic.fc
+        cr = self.critic.fc
         out = dict(values=self._tmp("ea_values", (B,), dev), log_probs=self._tmp("ea_lp", (B,), dev),
                    entropy=self._tmp("ea_ent", (B,), dev), metrics=self._tmp("ea_metrics", (ops.N_METRICS,), dev),
-                   d_features=self._tmp("d_features", (B, H), dev), d_w_act=ad.weight.grad, d_b_act=ad.bias.grad,
-                   d_w_val=cr.weight.grad, d_b_val=cr.bias.grad)
+                   d_features=self._tmp("d_features", (B, H), dev), d_w_val=cr.weight.grad, d_b_val=cr.bias.grad)
         f32 = lambda t: t.reshape(-1).contiguous()  # noqa: E731
-        ops.ppo_loss(feats, ad.weight, ad.bias, cr.weight, cr.bias, f32(batch["actions"]),
-                     f32(batch["action_log_probs"]), f32(batch["advantages"]), f32(batch["value_preds"]),
-                     f32(batch["returns"]), clip_param, value_loss_coef, entropy_coef, use_clipped_value_loss, True,
-                     out, self._loss_ws(B, dev), is_coeffs=f32(batch["is_coeffs"]) if "is_coeffs" in batch else None)
+        is_coeffs = f32(batch["is_coeffs"]) if "is_coeffs" in batch else None
+        if self._gaussian:
+            self._gaussian_loss(feats, batch["actions"], f32(batch["action_log_probs"]), f32(batch["advantages"]),
+                                f32(batch["value_preds"]), f32(batch["returns"]), clip_param, value_loss_coef,
+                                entropy_coef, use_clipped_value_loss, True, out, B, dev, is_coeffs=is_coeffs)
+        else:
+            ad = self.action_distribution.linear
+            out.update(d_w_act=ad.weight.grad, d_b_act=ad.bias.grad)
+            ops.ppo_loss(feats, ad.weight, ad.bias, cr.weight, cr.bias, f32(batch["actions"]),
+                         f32(batch["action_log_probs"]), f32(batch["advantages"]), f32(batch["value_preds"]),
+                         f32(batch["returns"]), clip_param, value_loss_coef, entropy_coef, use_clipped_value_loss, True,
+                         out, self._loss_ws(B, dev), is_coeffs=is_coeffs)
         d_rnn_in = self._rnn_backward(out["d_features"], s["layers"], s["masks"], T, n, B, dev)
         if self.tail_grads_hook is not None:
             with self._side.after_main():   # after the head gradients (main) and the RNN weight gradients (side)
@@ -1204,12 +1316,13 @@ class PointNavResNetPolicy(NativeNetPolicy):
                  aux_loss_config=None, fuse_keys=None, **kwargs):
         if force_blind_policy:
             raise NotImplementedError("force_blind_policy is not implemented")
-        if policy_config is not None and getattr(policy_config, "action_distribution_type", "categorical") != "categorical":
-            raise NotImplementedError("only categorical action distributions are implemented")
+        dist_type = "categorical"
+        if policy_config is not None:   # resnet_policy.py:84-94
+            dist_type = getattr(policy_config, "action_distribution_type", "categorical")
         super().__init__(PointNavResNetNet(observation_space, action_space, hidden_size, num_recurrent_layers,
                                            rnn_type, backbone, resnet_baseplanes, normalize_visual_inputs,
-                                           fuse_keys=fuse_keys),
-                         action_space)
+                                           fuse_keys=fuse_keys, discrete_actions=dist_type == "categorical"),
+                         action_space, dist_type, getattr(policy_config, "action_dist", None))
         self.observation_space = observation_space
         self._engines: Dict[str, EncoderEngine] = {}
 
@@ -1357,7 +1470,8 @@ class PointNavResNetPolicy(NativeNetPolicy):
         rnn_in = self._tmp("rnn_in", (B, Dp), dev)[:, :D]
         feats = {"visual": self._encode("visual", obs, rows, B, dev, train, rnn_in, 0)}
         segs = net.segments
-        if [sg["kind"] for sg in segs] == ["linear", "prev_action"] and segs[0]["transform"] == ops.T_POLAR2:
+        if (net.discrete_actions and [sg["kind"] for sg in segs] == ["linear", "prev_action"]
+                and segs[0]["transform"] == ops.T_POLAR2):
             # PointNav sensor set: goal embedding + prev-action embedding in one launch
             ops.embed_fwd(obs[POINTGOAL_UUID].reshape(-1, 2), pa, mk, rows, net.tgt_embeding.weight,
                           net.tgt_embeding.bias, net.prev_action_embedding.weight, rnn_in, H)
@@ -1377,6 +1491,9 @@ class PointNavResNetPolicy(NativeNetPolicy):
                     if idx.dtype != torch.int64:
                         idx = idx.long()
                     ops.index_embed_fwd(idx, rows, None, getattr(net, sg["attr"]).weight, rnn_in, col, B)
+                elif kind == "prev_action" and not net.discrete_actions:
+                    pe = net.prev_action_embedding
+                    ops.prev_action_linear_fwd(pa, mk, pe.weight, pe.bias, rnn_in, col)
                 elif kind == "prev_action":
                     ops.index_embed_fwd(pa, None, mk, net.prev_action_embedding.weight, rnn_in, col, B)
                 elif kind == "imagegoal":
@@ -1389,7 +1506,8 @@ class PointNavResNetPolicy(NativeNetPolicy):
         v = s["visual"]
         obs, rows, pa, mk = s["obs"], s["rows"], s["pa"], s["masks"]
         segs = net.segments
-        if [sg["kind"] for sg in segs] == ["linear", "prev_action"] and segs[0]["transform"] == ops.T_POLAR2:
+        if (net.discrete_actions and [sg["kind"] for sg in segs] == ["linear", "prev_action"]
+                and segs[0]["transform"] == ops.T_POLAR2):
             tg, emb = net.tgt_embeding, net.prev_action_embedding
             ops.embed_bwd(obs[POINTGOAL_UUID].reshape(-1, 2), pa, mk, rows, d_rnn_in, H, tg.weight.grad, tg.bias.grad,
                           emb.weight.grad)
@@ -1405,6 +1523,9 @@ class PointNavResNetPolicy(NativeNetPolicy):
                     idx = obs[sg["key"]].reshape(-1)
                     ops.index_embed_bwd(idx if idx.dtype == torch.int64 else idx.long(), rows, None, d_rnn_in, col,
                                         getattr(net, sg["attr"]).weight.grad, B)
+                elif kind == "prev_action" and not net.discrete_actions:
+                    pe = net.prev_action_embedding
+                    ops.prev_action_linear_bwd(pa, mk, d_rnn_in, col, pe.weight.grad, pe.bias.grad)
                 elif kind == "prev_action":
                     ops.index_embed_bwd(pa, None, mk, d_rnn_in, col, net.prev_action_embedding.weight.grad, B)
         # encoders: visual_fc (+ image-goal fc) -> conv stacks

@@ -81,6 +81,8 @@ class SingleAgentAccessMgr:
         if self._is_static_encoder:
             if getattr(hb, "force_blind_policy", False):
                 raise NotImplementedError("train_encoder=False with a blind policy: there is no visual encoder to freeze")
+            if getattr(hb.rl.policy[self.agent_name], "action_distribution_type", "categorical") != "categorical":
+                raise NotImplementedError("train_encoder=False with a gaussian action distribution is not implemented")
             if not issubclass(cls, PointNavResNetPolicy):
                 raise NotImplementedError(f"train_encoder=False is implemented for PointNavResNetPolicy only, not "
                                           f"{cls.__name__} (SimpleCNN)")

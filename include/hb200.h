@@ -108,6 +108,48 @@ int hb200_ppo_loss(const float* features, const float* w_act, const float* b_act
                    float* d_w_val, float* d_b_val, float* metrics, void* workspace,
                    hb200_stream_t stream);
 
+/* ---- Gaussian action head (continuous actions): act tail and PPO loss ----------------------------------------
+ * replaces GaussianNet + CustomNormal + CriticHead (HB/utils/common.py:99-175, HB/rl/ppo/policy.py:330-342, 416-424)
+ * and, for the loss, the same section of PPO._update_from_batch as hb200_ppo_loss (HB/rl/ppo/ppo.py:195-250).
+ *
+ * flags (ActionDistributionConfig): HB200_GAUSS_LOG_STD use_log_std, _SOFTPLUS use_softplus, _STD_PARAM use_std_param,
+ * _CLAMP_STD clamp_std, _TANH action_activation == "tanh".  min_std / max_std are the clamp bounds GaussianNet derives
+ * (min/max_log_std with use_log_std, inverse-softplus of min/max_std with use_softplus, else min/max_std).
+ * w_mu f32 [L,H], b_mu [L]: mu_maybe_std, L = A with use_std_param (std_param f32 [A], else NULL), 2A without it (rows
+ * [A, 2A) are the std outputs).  w_val [1,H], b_val [1] the critic.  std = softplus(exp(clamp(s))) with each step
+ * applied when its flag is set, in that order; mu = tanh(mu) with _TANH.  1 <= A <= 16, H in {32, 64, 128, 256, 512};
+ * anything else is refused with an argument error before any launch.
+ */
+#define HB200_GAUSS_LOG_STD 1
+#define HB200_GAUSS_SOFTPLUS 2
+#define HB200_GAUSS_STD_PARAM 4
+#define HB200_GAUSS_CLAMP_STD 8
+#define HB200_GAUSS_TANH 16
+#define HB200_GAUSS_ALL_FLAGS 31
+/* Policy.act's tail in one launch: actions f32 [B,A] = mu + eps * std (CustomNormal.rsample; eps f32 [B,A] drawn by the
+ * caller) or mu when eps == NULL (deterministic: distribution.mean); action_log_probs f32 [B] = Normal log_prob summed
+ * over the action dimensions; values f32 [B].  Graph-capturable (no allocation, no host synchronisation). */
+int hb200_gaussian_act(const float* features, const float* w_mu, const float* b_mu, const float* std_param,
+                       const float* w_val, const float* b_val, const float* eps, int batch, int hidden, int n_actions,
+                       int flags, float min_std, float max_std, float* actions, float* action_log_probs, float* values,
+                       hb200_stream_t stream);
+/* Forward + backward like hb200_ppo_loss, for actions f32 [B,A]: the same outputs and the same 12 metrics; log_probs and
+ * entropy are the per-frame sums over the action dimensions.  Gradients (OVERWRITTEN): d_features [B,H], d_w_mu [L,H],
+ * d_b_mu [L], d_std [A] (use_std_param only, else may be NULL), d_w_val [H], d_b_val [1].  Frame sums are per-slab
+ * partials added in a fixed order (no floating-point atomics): the same result every run.  At its bounds the clamp
+ * passes the gradient; softplus's backward switches to the identity above 20, as torch's does.  NaN reaches what it
+ * reaches in the reference's autograd (a NaN raw std below the clamp has gradient 0, as torch.clamp's backward gives).
+ * workspace: hb200_gaussian_ppo_loss_workspace_bytes(B,H,A). */
+size_t hb200_gaussian_ppo_loss_workspace_bytes(int batch, int hidden, int n_actions);
+int hb200_gaussian_ppo_loss(const float* features, const float* w_mu, const float* b_mu, const float* std_param,
+                            const float* w_val, const float* b_val, const float* actions, const float* old_log_probs,
+                            const float* advantages, const float* old_values, const float* returns,
+                            const float* is_coeffs, int batch, int hidden, int n_actions, int flags, float min_std,
+                            float max_std, float clip_param, float value_loss_coef, float entropy_coef,
+                            int use_clipped_value_loss, int compute_grads, float* values, float* log_probs,
+                            float* entropy, float* d_features, float* d_w_mu, float* d_b_mu, float* d_std,
+                            float* d_w_val, float* d_b_val, float* metrics, void* workspace, hb200_stream_t stream);
+
 /* ---- clip_grad_norm_ + Adam on flat buffers ---------------------------------------
  * replaces nn.utils.clip_grad_norm_ + torch.optim.Adam(foreach=True).step()
  * (HB/rl/ppo/ppo.py:112-137, 257, 347-371).
@@ -512,6 +554,13 @@ int hb200_index_embed_fwd(const int64_t* idx, const int32_t* frame_rows, const u
 int hb200_index_embed_bwd(const int64_t* idx, const int32_t* frame_rows, const uint8_t* masks, int batch,
                           int table_rows, int width, const float* d_out, int ld, int col0, float* d_table,
                           hb200_stream_t stream);
+/* Continuous previous action (resnet_policy.py:420-428, 755-757): out[f, col0 + j] = b[j] + sum_k w[j, k] m_f pa[f, k]
+ * with pa f32 [batch, n_actions], masks u8 [batch], w f32 [32, n_actions] (nn.Linear(A, 32)), 1 <= n_actions <= 64.
+ * _bwd adds to d_w / d_b; frames are summed in a fixed order (per-chunk partials, then reduce_partials). */
+int hb200_prev_action_linear_fwd(const float* prev_actions, const uint8_t* masks, int batch, int n_actions,
+                                 const float* w, const float* b, float* out, int ld, int col0, hb200_stream_t stream);
+int hb200_prev_action_linear_bwd(const float* prev_actions, const uint8_t* masks, int batch, int n_actions,
+                                 const float* d_out, int ld, int col0, float* d_w, float* d_b, hb200_stream_t stream);
 /* Generic visual input prep (ResNetEncoder.forward, HB/rl/ddppo/policy/resnet_policy.py:255-271) for ANY sensor mix
  * and size: up to 4 HWC sources (h_* are HOST arrays of n_srcs entries: device pointers, dtype 0 u8 / 1 f32 / 2 i32,
  * channels, pre-pool scale = 1/high for u8 keys), <= 8 channels in total, concatenated in order, avg_pool2d(2) (odd

@@ -20,6 +20,8 @@ _LAZY = {
     "FusedAdam": ("rl.ppo", "FusedAdam"),
     "RolloutStorage": ("common.rollout_storage", "RolloutStorage"),
     "PPOTrainer": ("rl.ppo_trainer", "PPOTrainer"),
+    "VERTrainer": ("rl.ver_trainer", "VERTrainer"),
+    "VERRolloutStorage": ("common.ver_rollout_storage", "VERRolloutStorage"),
     "SingleAgentAccessMgr": ("rl.single_agent_access_mgr", "SingleAgentAccessMgr"),
     "ddp_utils": ("rl.ddp_utils", None),
     "GraphedActor": ("rl.graphed_actor", "GraphedActor"),

@@ -18,6 +18,7 @@ _C = {
     "i": ctypes.c_int,
     "l": ctypes.c_longlong,
     "f": ctypes.c_float,
+    "d": ctypes.c_double,
     "z": ctypes.c_size_t,
     "s": ctypes.c_char_p,
 }
@@ -28,6 +29,7 @@ SIGNATURES = {
     "hb200_version": ("i", ""),
     "hb200_launch_count": ("l", ""),
     "hb200_gae_adv": ("i", "ppppppp" + "iii" + "ff" + "ii" + "p"),
+    "hb200_ver_gae": ("i", "ppppp" + "iii" + "dd" + "i" + "pp" + "i" + "p"),
     "hb200_adv_normalize": ("i", "plppip"),
     "hb200_ppo_loss_workspace_bytes": ("z", "iii"),
     "hb200_ppo_loss": ("i", "ppppppppppp" + "iii" + "fff" + "ii" + "ppp" + "ppppp" + "ppp"),
@@ -92,6 +94,7 @@ SIGNATURES = {
     "hb200_colsum": ("i", "plplii" + "p"),
     "hb200_relu_bwd": ("i", "pplll" + "i" + "p"),
     "hb200_gather_rows": ("i", "pppil" + "p"),
+    "hb200_gather_rows_pad": ("i", "plppl" + "ii" + "p"),
     "hb200_f32_chw_to_bf16_hwc": ("i", "pp" + "iii" + "p"),
     "hb200_heads_fwd": ("i", "ppppp" + "iii" + "pp" + "p"),
     "hb200_heads_act": ("i", "pppppp" + "iii" + "pppp" + "p"),

@@ -2711,3 +2711,29 @@ extern "C" int hb200_gather_rows(const float* src, const int32_t* frame_rows, fl
   count_launch(1);
   return HB200_OK;
 }
+
+// ======================================================================================
+// VER learner: rows between the minibatch's frame order and the recurrence's time-major [T_max, S] layout
+// ======================================================================================
+namespace hb200 {
+__global__ void gather_rows_pad_kernel(const float* __restrict__ src, long long ld_src, const int32_t* __restrict__ idx,
+                                       float* __restrict__ out, long long ld_out, int rows, int cols) {
+  const long long total = (long long)rows * cols;
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    const long long r = i / cols, c = i - r * cols;
+    const int j = idx[r];
+    out[r * ld_out + c] = j >= 0 ? __ldg(src + (long long)j * ld_src + c) : 0.f;
+  }
+}
+}  // namespace hb200
+
+extern "C" int hb200_gather_rows_pad(const float* src, long long ld_src, const int32_t* idx, float* out,
+                                     long long ld_out, int rows, int cols, hb200_stream_t stream) {
+  HB_CHECK_ARG(src && idx && out && rows > 0 && cols > 0 && ld_src >= cols && ld_out >= cols,
+               "gather_rows_pad: bad args rows=%d cols=%d ld_src=%lld ld_out=%lld", rows, cols, ld_src, ld_out);
+  gather_rows_pad_kernel<<<grid_for((long long)rows * cols, 256), 256, 0, (cudaStream_t)stream>>>(
+      src, ld_src, idx, out, ld_out, rows, cols);
+  HB_LAUNCH_OK();
+  count_launch(1);
+  return HB200_OK;
+}

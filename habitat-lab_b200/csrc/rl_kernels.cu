@@ -246,6 +246,93 @@ extern "C" int hb200_gae_adv(const float* rewards, float* value_preds, const uin
   return HB200_OK;
 }
 
+// =====================================================================================
+// VER: GAE over packed sequences (HB/rl/ver/ver_rollout_storage.py:430-568) + advantages
+// =====================================================================================
+// Step t of sequence s is frame select_inds[step_offset[t] + s]; sequences are sorted by length, longest first.
+// One thread walks one sequence backwards, in fp64 with unfused operations in the reference's (numpy) order, so every
+// return is the reference's float64 value rounded once to fp32: the results are bit-identical to it.  After a block
+// barrier the same block writes advantages = returns - value_preds for every frame and sums the finite ones in a fixed
+// order (one block: the statistics do not depend on scheduling).
+constexpr int kVerGaeThreads = 1024;
+__global__ void __launch_bounds__(kVerGaeThreads)
+ver_gae_kernel(const float* __restrict__ rewards, const float* __restrict__ values, float* __restrict__ returns,
+               const uint8_t* __restrict__ is_stale, const int32_t* __restrict__ select_inds,
+               const int32_t* __restrict__ step_offset, const int32_t* __restrict__ seq_len,
+               const int32_t* __restrict__ last_for_env, int n_frames, int n_seqs, double gamma, double gt,
+               float* __restrict__ adv, double* __restrict__ stats) {
+  __shared__ double red[32];
+  for (int s = threadIdx.x; s < n_seqs; s += blockDim.x) {
+    const bool env_last = last_for_env[s] != 0;
+    double gae = 0.0, last_v = 0.0;
+    for (int t = seq_len[s] - 1; t >= 0; --t) {
+      const int i = select_inds[step_offset[t] + s];
+      const double v = (double)values[i];
+      const double delta = __dsub_rn(__dadd_rn((double)rewards[i], __dmul_rn(gamma, last_v)), v);
+      gae = __dadd_rn(delta, __dmul_rn(gt, gae));
+      const bool bootstrap = env_last && t == seq_len[s] - 1;
+      if (bootstrap) gae = 0.0;   // the bootstrap step only provides last_v for the step before it
+      const float old = returns[i];
+      if (bootstrap) {
+        returns[i] = __int_as_float(0x7fc00000);
+      } else if (!is_stale[i] || !isfinite(old)) {
+        returns[i] = (float)__dadd_rn(gae, v);
+      }
+      last_v = v;
+    }
+  }
+  __syncthreads();
+  double s = 0, ss = 0, cnt = 0, fin = 0;
+  for (int i = threadIdx.x; i < n_frames; i += blockDim.x) {
+    const float r = returns[i];
+    const float a = __fsub_rn(r, values[i]);
+    if (adv) adv[i] = a;
+    acc_stats(a, s, ss, cnt);
+    fin += isfinite(r) ? 1.0 : 0.0;
+  }
+  s = block_sum(s, red);
+  ss = block_sum(ss, red);
+  cnt = block_sum(cnt, red);
+  fin = block_sum(fin, red);
+  if (threadIdx.x == 0 && stats) {
+    stats[0] = s;
+    stats[1] = ss;
+    stats[2] = cnt;
+    stats[3] = fin;
+  }
+}
+
+extern "C" int hb200_ver_gae(const float* rewards, const float* value_preds, float* returns, const uint8_t* is_stale,
+                             const int32_t* seq_table, int n_frames, int n_seqs, int max_len, double gamma, double tau,
+                             int use_gae, float* advantages, double* stats, int expected_finite,
+                             hb200_stream_t stream) {
+  HB_CHECK_ARG(rewards && value_preds && returns && is_stale && seq_table && stats, "ver_gae: null pointer");
+  HB_CHECK_ARG(n_frames > 0 && n_seqs > 0 && n_seqs <= n_frames && max_len > 0 && max_len <= n_frames,
+               "ver_gae: bad sizes n_frames=%d n_seqs=%d max_len=%d", n_frames, n_seqs, max_len);
+  cudaStream_t st = (cudaStream_t)stream;
+  const int32_t* select_inds = seq_table;
+  const int32_t* step_offset = seq_table + n_frames;
+  const int32_t* seq_len = step_offset + max_len;
+  const int32_t* last_for_env = seq_len + n_seqs;
+  // the reference evaluates `gamma * last_values` and `(tau * gamma) * gae` with python floats: double throughout
+  const double g = gamma, gt = (use_gae ? tau : 1.0) * g;
+  ver_gae_kernel<<<1, kVerGaeThreads, 0, st>>>(rewards, value_preds, returns, is_stale, select_inds, step_offset,
+                                              seq_len, last_for_env, n_frames, n_seqs, g, gt, advantages, stats);
+  HB_LAUNCH_OK();
+  count_launch(1);
+  if (expected_finite >= 0) {   // the reference's invariant: exactly T * N finite returns (one NaN bootstrap per env)
+    double fin = 0;
+    HB_CUDA(cudaMemcpyAsync(&fin, stats + 3, sizeof(double), cudaMemcpyDeviceToHost, st));
+    HB_CUDA(cudaStreamSynchronize(st));
+    if ((long long)fin != (long long)expected_finite) {
+      set_last_error("ver_gae: %lld finite returns, expected %d (one bootstrap step per environment)",
+                     (long long)fin, expected_finite);
+      return HB200_ERR_INVALID_ARG;
+    }
+  }
+  return HB200_OK;
+}
+
 __global__ void adv_normalize_kernel(float* __restrict__ adv, long long n,
                                      const double* __restrict__ stats,
                                      const float* __restrict__ mean_var, int mode) {

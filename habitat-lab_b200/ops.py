@@ -42,6 +42,37 @@ def gae_adv(rewards, value_preds, masks, next_value, returns, advantages, stats,
          int(bool(use_gae)), int(variant))
 
 
+def ver_gae(rewards, value_preds, returns, is_stale, seq_table, n_seqs, max_len, gamma, tau, use_gae, advantages,
+            stats, expected_finite=-1):
+    """GAE over packed sequences (include/hb200.h hb200_ver_gae): flat f32 rewards / value_preds / returns (in/out) /
+    advantages, bool is_stale, int32 seq_table; stats f64[4]."""
+    M = rewards.numel()
+    for t, nm in ((rewards, "rewards"), (value_preds, "value_preds"), (returns, "returns"), (advantages, "advantages")):
+        _chk(t, torch.float32, nm)
+        if t.numel() != M:
+            raise _lib.Hb200Error(f"ver_gae: {nm} has {t.numel()} elements, expected {M}")
+    if is_stale.numel() != M or not is_stale.is_cuda or not is_stale.is_contiguous() or is_stale.element_size() != 1:
+        raise _lib.Hb200Error(f"ver_gae: is_stale must be a contiguous 1-byte CUDA tensor of {M} elements")
+    _chk(seq_table, torch.int32, "seq_table")
+    _chk(stats, torch.float64, "stats")
+    if seq_table.numel() != M + max_len + 2 * n_seqs:
+        raise _lib.Hb200Error("ver_gae: seq_table size does not match n_frames + max_len + 2 * n_seqs")
+    call("hb200_ver_gae", ptr(rewards), ptr(value_preds), ptr(returns), ptr(as_u8(is_stale)), ptr(seq_table), int(M),
+         int(n_seqs), int(max_len), float(gamma), float(tau), int(bool(use_gae)), ptr(advantages), ptr(stats),
+         int(expected_finite))
+
+
+def gather_rows_pad(src, idx, out):
+    """out[r] = src[idx[r]] (idx[r] >= 0) or 0: f32 2-D views with unit column stride, int32 idx."""
+    _chk(idx, torch.int32, "idx")
+    if src.stride(1) != 1 or out.stride(1) != 1 or src.shape[1] != out.shape[1] or idx.numel() != out.shape[0]:
+        raise _lib.Hb200Error("gather_rows_pad: expected row-major f32 views of equal width and one index per row")
+    if src.dtype != torch.float32 or out.dtype != torch.float32:
+        raise _lib.Hb200Error("gather_rows_pad: expected float32")
+    call("hb200_gather_rows_pad", ptr(src), src.stride(0), ptr(idx), ptr(out), out.stride(0), out.shape[0],
+         out.shape[1])
+
+
 def adv_normalize(advantages, stats=None, mean_var=None):
     mode = 0 if mean_var is None else 1
     call("hb200_adv_normalize", ptr(advantages), advantages.numel(), ptr(stats), ptr(mean_var), mode)

@@ -169,6 +169,9 @@ class PPO(nn.Module):
         learner_metrics["_metrics"].append(metrics.clone())
         learner_metrics["grad_norm"].append(grad_norm.clone())
         learner_metrics["_is_last_epoch"].append(epoch == (self.ppo_epoch - 1))
+        if "is_coeffs" in batch:   # VER's importance weights, unclamped (ppo.py:261-262)
+            isc = batch["is_coeffs"].reshape(-1)
+            learner_metrics["_ver_is_coeffs"].append(torch.stack([isc.min(), isc.mean(), isc.max()]))
 
     def before_step(self) -> torch.Tensor:
         """all-reduce (distributed) + clip_grad_norm_ + Adam, fused (ppo.py:347-371, 257-258)."""
@@ -212,10 +215,15 @@ class PPO(nn.Module):
         gn = torch.stack(lm["grad_norm"]).reshape(-1, 1)
         last = torch.tensor(lm["_is_last_epoch"], device=m.device).view(-1, 1).float()
         frac = (m[:, 9:10] * last).sum() / last.sum().clamp(min=1)  # ppo_fraction_clipped: last epoch only
-        host = torch.cat([m.mean(0), gn.mean(0), frac.view(1)]).cpu().tolist()
+        parts = [m.mean(0), gn.mean(0), frac.view(1)]
+        if lm.get("_ver_is_coeffs"):
+            parts.append(torch.stack(lm["_ver_is_coeffs"]).mean(0))
+        host = torch.cat(parts).cpu().tolist()
         out = {k: host[i] for i, k in enumerate(ops.METRIC_KEYS[:9])}
         out["ppo_fraction_clipped"] = host[13]
         out["grad_norm"] = host[12]
+        if len(host) > 14:
+            out.update(ver_is_coeffs_min=host[14], ver_is_coeffs_mean=host[15], ver_is_coeffs_max=host[16])
         return out
 
     def _evaluate_actions(self, *args, **kwargs):

@@ -74,15 +74,26 @@ class DDPPOConfig:
     force_distributed: bool = False
 
 
+@dataclass
+class VERConfig:
+    variable_experience: bool = True
+    num_inference_workers: int = 2
+    overlap_rollouts_and_learn: bool = False
+
+
 def make_config(num_environments=4, total_num_steps=-1.0, num_updates=2, height=256, width=256, seed=100,
-                obs_transforms=None, ddppo=None, continuous_actions=0, action_dist=None, **ppo_kw):
+                obs_transforms=None, ddppo=None, continuous_actions=0, action_dist=None, trainer_name="ddppo",
+                ver=None, step_time_spread=0.0, **ppo_kw):
     """A habitat_baselines-shaped config for the synthetic PointNav DD-PPO run (ddppo_pointnav.yaml values).
     obs_transforms: {name: config node with `type` and the transformer's fields} (e.g. the ObjectNav YAMLs'
     resize_shortest_edge + center_cropper, common/obs_transformers.py); height / width are then the raw sensor size.
     ddppo: DDPPOConfig field overrides, e.g. dict(pretrained=True, pretrained_weights=path, train_encoder=False).
     continuous_actions = A > 0: continuous control -- a Box(-1, 1, (A,)) action space and the gaussian policy
     (monolithic.yaml), with action_dist the ActionDistributionConfig field overrides (e.g. social_nav.yaml's
-    dict(use_std_param=True))."""
+    dict(use_std_param=True)).
+    trainer_name="ver": Variable Experience Rollout (rl/ver_trainer.py) with `ver` the VERConfig field overrides;
+    step_time_spread > 0 gives every synthetic environment step its own duration on a seeded virtual clock, so
+    environments contribute unequal numbers of steps to a rollout."""
     ppo = PPOConfig(**{**dict(ppo_epoch=2, num_mini_batch=2, num_steps=128, max_grad_norm=0.2), **ppo_kw})
     agent = SimpleNamespace(name="PointNavResNetPolicy", action_distribution_type="categorical")
     if continuous_actions:
@@ -91,16 +102,18 @@ def make_config(num_environments=4, total_num_steps=-1.0, num_updates=2, height=
     if obs_transforms is not None:
         agent.obs_transforms = dict(obs_transforms)
     hb = SimpleNamespace(
-        trainer_name="ddppo", updater_name="PPO", distrib_updater_name="DDPPO", rollout_storage_name="RolloutStorage",
+        trainer_name=trainer_name, updater_name="PPO", distrib_updater_name="DDPPO", rollout_storage_name="RolloutStorage",
         num_environments=num_environments, total_num_steps=total_num_steps, num_updates=num_updates,
         log_interval=10, force_blind_policy=False, num_checkpoints=-1, checkpoint_interval=-1,
         checkpoint_folder="data/checkpoints",
-        rl=SimpleNamespace(ppo=ppo, ddppo=DDPPOConfig(**(ddppo or {})), policy={"main_agent": agent}),
+        rl=SimpleNamespace(ppo=ppo, ddppo=DDPPOConfig(**(ddppo or {})), policy={"main_agent": agent},
+                           ver=VERConfig(**(ver or {}))),
         eval=SimpleNamespace(extra_sim_sensors={}),
     )
     habitat = SimpleNamespace(seed=seed, simulator=SimpleNamespace(agents_order=["main_agent"]),
                               synthetic=SimpleNamespace(height=height, width=width, p_done=1.0 / 250.0,
-                                                        continuous_actions=int(continuous_actions)))
+                                                        continuous_actions=int(continuous_actions),
+                                                        step_time_spread=float(step_time_spread)))
     return SimpleNamespace(habitat_baselines=hb, habitat=habitat)
 
 
@@ -109,7 +122,7 @@ class SyntheticVectorEnv:
     """VectorEnv-shaped source of synthetic RGB-D PointNav observations born on the device
     (method surface: habitat/core/vector_env.py as used by ppo_trainer.py:136-157, 266-267, 388, 409-419)."""
 
-    def __init__(self, num_envs, obs_space, act_space, device, seed, p_done):
+    def __init__(self, num_envs, obs_space, act_space, device, seed, p_done, step_time_spread=0.0):
         self.num_envs = num_envs
         self.observation_spaces = [obs_space] * num_envs
         self.action_spaces = [act_space] * num_envs
@@ -118,11 +131,20 @@ class SyntheticVectorEnv:
         self.gen = torch.Generator(device=device).manual_seed(seed)
         self.p_done = p_done
         self._pending = None
+        # opt-in: every step of every environment takes 1 + spread * U[0, 1) time units on a virtual clock, drawn from
+        # a generator of its own so the observation / reward stream is the same with or without it
+        self.step_time_spread = float(step_time_spread)
+        self.clock = np.random.default_rng(seed)
 
-    def _obs(self):
+    def step_durations(self, n: int) -> np.ndarray:
+        if self.step_time_spread <= 0.0:
+            return np.ones(n)
+        return 1.0 + self.step_time_spread * self.clock.random(n)
+
+    def _obs(self, n=None):
         sp = self.observation_spaces[0].spaces
         out = {}
-        n, d, g = self.num_envs, self.device, self.gen
+        n, d, g = self.num_envs if n is None else n, self.device, self.gen
         if "rgb" in sp:
             out["rgb"] = torch.randint(0, 256, (n, *sp["rgb"].shape), generator=g, device=d, dtype=torch.uint8)
         if "depth" in sp:
@@ -136,12 +158,13 @@ class SyntheticVectorEnv:
     def reset(self):
         return self._obs()
 
-    def step(self, actions):
-        """Batched step: (obs dict, rewards [N,1], dones [N] bool, infos)."""
-        n, d, g = self.num_envs, self.device, self.gen
+    def step(self, actions, n=None):
+        """Batched step: (obs dict, rewards [N,1], dones [N] bool, infos).  n: step only that many environments (the
+        VER trainer steps the ones whose previous step has completed)."""
+        n, d, g = self.num_envs if n is None else n, self.device, self.gen
         dones = torch.rand(n, generator=g, device=d) < self.p_done
         rewards = torch.randn(n, 1, generator=g, device=d) * 0.1 + 2.5 * dones.float().view(n, 1)
-        return self._obs(), rewards, dones, [{} for _ in range(n)]
+        return self._obs(n), rewards, dones, [{} for _ in range(n)]
 
     # -- the per-environment surface the REFERENCE's trainer drives (ppo_trainer.py:388, 409-419, 266-267):
     #    async_step_at(i, a) for every env of a buffer, then wait_step_at(i) -> (obs, reward, done, info), post_step(obs)
@@ -180,7 +203,8 @@ class SyntheticVectorEnvFactory:
         if getattr(syn, "continuous_actions", 0):   # the environment draws no random numbers for its actions
             act_space = spaces.Box(-1.0, 1.0, (syn.continuous_actions,), np.float32)
         n = config.habitat_baselines.num_environments
-        return SyntheticVectorEnv(n, obs_space, act_space, device, config.habitat.seed + rank * n, syn.p_done)
+        return SyntheticVectorEnv(n, obs_space, act_space, device, config.habitat.seed + rank * n, syn.p_done,
+                                  getattr(syn, "step_time_spread", 0.0))
 
 
 # ---- the trainer -------------------------------------------------------------------------------------------
@@ -249,7 +273,7 @@ class PPOTrainer:
         self._agent = self._create_agent(None)
         if torch.distributed.is_initialized():
             self._agent.init_distributed(find_unused_params=False)
-        self._agent.post_init()
+        self._agent.post_init(self._rollouts_factory())
         obs = self.envs.reset()
         if self._obs_plan:
             rest = self._obs_plan.apply_(obs, self.rollouts.buffers["observations"][0])
@@ -278,6 +302,10 @@ class PPOTrainer:
         t0 = time.perf_counter()
         self.actor_critic.encode_visual_features(obs[slot], obs[VISUAL_FEATURES_KEY][slot])
         self.timings["visual_features"] += time.perf_counter() - t0
+
+    def _rollouts_factory(self):
+        """create_rollouts_fn for SingleAgentAccessMgr.post_init: None builds the configured rollout storage."""
+        return None
 
     def _create_obs_transforms(self):
         """ppo_trainer.py:110-113: the policy and the storage are built for the transformed observation space.  The
@@ -436,3 +464,6 @@ class PPOTrainer:
             self._last_fps = self.num_steps_done / max(time.time() - self.t_start, 1e-9)
         self.envs.close()
         return losses
+
+
+from . import ver_trainer  # noqa: E402,F401  (registers the "ver" trainer)

@@ -15,6 +15,7 @@ There is no CPU / PyTorch fallback: tensors must live on a CUDA device.
 """
 from __future__ import annotations
 
+import contextlib
 import math
 import os
 from collections import OrderedDict
@@ -1167,23 +1168,97 @@ class NativeNetPolicy(nn.Module):
         return dxs[0]
 
     # ---- shared forward ----------------------------------------------------------------------------------
-    def _trunk(self, observations, rnn_hidden_states, prev_actions, masks, train: bool):
+    def _trunk(self, observations, rnn_hidden_states, prev_actions, masks, train: bool, seq=None):
         obs, rows = _as_rows(observations, rnn_hidden_states.device)
         dev = rnn_hidden_states.device
         if dev.type != "cuda":
             raise Hb200Error("hb200 policy: inputs must be CUDA tensors (no CPU fallback)")
         self.flatten_parameters_()
         B = rows.numel()
-        n = rnn_hidden_states.shape[0]
-        T = B // n
-        assert T * n == B, "frames must be (t, env)-ordered with T*n rows"
+        if seq is not None:
+            self._check_packed_columns(seq.num_seqs)
+        n = rnn_hidden_states.shape[0] if seq is None else seq.num_seqs
+        T = B // n if seq is None else seq.max_len
+        assert seq is not None or T * n == B, "frames must be (t, env)-ordered with T*n rows"
         pa = prev_actions.reshape(B, -1).contiguous() if self._gaussian else prev_actions.reshape(-1)
         mk = ops.as_u8(masks.reshape(-1))
         rnn_in, vsaved = self._visual_forward(obs, rows, pa, mk, B, dev, train)
         hid = rnn_hidden_states.contiguous()
-        feats, layers, hidden_out = self._rnn_forward(rnn_in, hid, mk, T, n, B, dev, train)
+        if seq is None:
+            feats, layers, hidden_out = self._rnn_forward(rnn_in, hid, mk, T, n, B, dev, train)
+        else:
+            feats, layers, hidden_out = self._packed_rnn_forward(rnn_in, hid, mk, seq, B, dev, train)
         return dict(B=B, n=n, T=T, rows=rows, obs=obs, masks=mk, pa=pa, layers=layers, features=feats,
-                    hidden_out=hidden_out, visual=vsaved)
+                    hidden_out=hidden_out, visual=vsaved, seq=seq)
+
+    # ---- recurrence over packed sequences (VER minibatches) -----------------------------------------------
+    # The S sequences of unequal length run time-major over [T_max, S]: the RNN input rows are scattered there with
+    # zero padding after each sequence's end, the unchanged sequence kernels run with every mask set (each sequence is
+    # one episode) from each sequence's own initial state, and the output rows are gathered back.  Padding steps come
+    # after every real step of their column, so they never feed one; in the backward they receive a zero output
+    # gradient and carry exact zeros, so they add nothing to any weight gradient.
+    def _packed_column_limit(self) -> int:
+        """Largest S the backward sequence kernels take (their per-CTA shared memory: rnn.cu lstm_seq_bwd / gru_seq_bwd)"""
+        rnn = self.net.state_encoder.rnn
+        H = rnn.hidden_size
+        floats = 200 * 1024 // 4
+        return (floats - 16 * H) // 8 if isinstance(rnn, nn.LSTM) else (floats - 12 * H) // 4
+
+    def _check_packed_columns(self, S: int) -> None:
+        if S > self._packed_column_limit():
+            raise Hb200Error(f"packed minibatch of {S} sequences: the recurrence backward takes at most "
+                             f"{self._packed_column_limit()} (use more minibatches)")
+
+    def _packed_rnn_forward(self, rnn_in, hid, mk, seq, B, dev, train):
+        rnn = self.net.state_encoder.rnn
+        H, L = rnn.hidden_size, rnn.num_layers
+        lstm = isinstance(rnn, nn.LSTM)
+        T, S = seq.max_len, seq.num_seqs
+        Bp = T * S
+        with self._packed_scope(T, S):
+            x_tm = self._tmp("packed_rnn_in", (Bp, rnn_in.stride(0)), dev)[:, : rnn_in.shape[1]]
+            mk_tm = self._tmp("packed_masks", (Bp,), dev, torch.uint8)
+        ops.gather_rows_pad(rnn_in, seq.tm_to_frame, x_tm)
+        mk_tm.fill_(1)
+        # initial state of each sequence: its environment's stored state, zeroed where the sequence starts an episode
+        keep = mk.index_select(0, seq.sequence_starts).to(hid.dtype).view(S, 1, 1)
+        hid_seq = (hid.index_select(0, seq.rnn_state_batch_inds) * keep).contiguous()
+        with self._packed_scope(T, S):
+            out_tm, layers, _ = self._rnn_forward(x_tm, hid_seq, mk_tm, T, S, Bp, dev, train)
+        feats = self._tmp("packed_features", (B, H), dev)
+        ops.gather_rows_pad(out_tm, seq.frame_to_tm, feats)
+        # each environment's state after its last sequence (the reference's build_rnn_out_from_seq)
+        last = seq.last_sequence_in_batch_inds
+        t_end = seq.sequence_lengths.index_select(0, last) - 1
+        parts = [ly["hs"][t_end, last] for ly in layers] + ([ly["cs"][t_end, last] for ly in layers] if lstm else [])
+        return feats, dict(layers=layers, mk=mk_tm), torch.stack(parts, dim=1)
+
+    @contextlib.contextmanager
+    def _packed_scope(self, T, S):
+        """The recurrence's scratch buffers of a packed minibatch live in their own cache, kept for one (T_max, S) at a
+        time: those shapes change from minibatch to minibatch, and caching every one would hold memory without bound.
+        (The frame count B of a VER minibatch takes at most two values per run, so per-frame buffers stay cached.)"""
+        if getattr(self, "_packed_key", None) != (T, S):
+            self._packed_key, self._packed_buf = (T, S), {}
+        outer, self._buf = self._buf, self._packed_buf
+        try:
+            yield
+        finally:
+            self._buf = outer
+
+    def _packed_rnn_backward(self, d_feats, packed, seq, B, dev):
+        T, S = seq.max_len, seq.num_seqs
+        Bp = T * S
+        H = d_feats.shape[1]
+        with self._packed_scope(T, S):
+            d_tm = self._tmp("packed_d_features", (Bp, H), dev)
+            ops.gather_rows_pad(d_feats, seq.tm_to_frame, d_tm)
+            d_in_tm = self._rnn_backward(d_tm, packed["layers"], packed["mk"], T, S, Bp, dev)
+        D = d_in_tm.shape[1]
+        Dp = (D + 3) // 4 * 4
+        d_in = self._tmp("packed_d_rnn_in", (B, Dp), dev)[:, :D]
+        ops.gather_rows_pad(d_in_tm, seq.frame_to_tm, d_in)
+        return d_in
 
     def _heads(self, feats, B, dev):
         values = self._tmp("values_act", (B,), dev)
@@ -1248,9 +1323,10 @@ class NativeNetPolicy(nn.Module):
     def evaluate_actions(self, observations, rnn_hidden_states, prev_actions, masks, action,
                          rnn_build_seq_info=None):
         """Forward only (values, log-probs, entropy, hidden, aux) like the reference
-        (rl/ppo/policy.py:361-402); `rnn_build_seq_info` is accepted and ignored: the masked
-        recurrence needs only `masks`."""
-        s = self._trunk(observations, rnn_hidden_states, prev_actions, masks, train=True)
+        (rl/ppo/policy.py:361-402).  Without `rnn_build_seq_info` the frames are a (t, env) rectangle and the masked
+        recurrence needs only `masks`; with it (a VER minibatch, common/ver_rollout_storage.PackedSequenceInfo) the
+        recurrence runs over its packed sequences and rnn_hidden_states holds one state per environment."""
+        s = self._trunk(observations, rnn_hidden_states, prev_actions, masks, train=True, seq=rnn_build_seq_info)
         feats, B = s["features"], s["B"]
         dev = feats.device
         out = dict(values=self._tmp("ea_values", (B,), dev), log_probs=self._tmp("ea_lp", (B,), dev),
@@ -1272,7 +1348,9 @@ class NativeNetPolicy(nn.Module):
         total_loss.backward() (rl/ppo/ppo.py:180-254).  Leaves every parameter's gradient in the flat
         gradient buffer (p.grad views) and returns the 12 metrics as a device tensor."""
         obs = observations if observations is not None else batch["observations"]
-        s = self._trunk(obs, batch["recurrent_hidden_states"], batch["prev_actions"], batch["masks"], train=True)
+        seq = batch.get("rnn_build_seq_info")
+        s = self._trunk(obs, batch["recurrent_hidden_states"], batch["prev_actions"], batch["masks"], train=True,
+                        seq=seq)
         feats, B, n, T = s["features"], s["B"], s["n"], s["T"]
         dev = feats.device
         H = self.net.output_size
@@ -1294,7 +1372,10 @@ class NativeNetPolicy(nn.Module):
                          f32(batch["action_log_probs"]), f32(batch["advantages"]), f32(batch["value_preds"]),
                          f32(batch["returns"]), clip_param, value_loss_coef, entropy_coef, use_clipped_value_loss, True,
                          out, self._loss_ws(B, dev), is_coeffs=is_coeffs)
-        d_rnn_in = self._rnn_backward(out["d_features"], s["layers"], s["masks"], T, n, B, dev)
+        if seq is None:
+            d_rnn_in = self._rnn_backward(out["d_features"], s["layers"], s["masks"], T, n, B, dev)
+        else:
+            d_rnn_in = self._packed_rnn_backward(out["d_features"], s["layers"], seq, B, dev)
         if self.tail_grads_hook is not None:
             with self._side.after_main():   # after the head gradients (main) and the RNN weight gradients (side)
                 self.tail_grads_hook()

@@ -128,6 +128,9 @@ class SingleAgentAccessMgr:
 
     def post_init(self, create_rollouts_fn: Optional[Callable] = None):
         hb = self._config.habitat_baselines
+        if create_rollouts_fn is not None:   # the trainer builds its own storage (ver_trainer.py's VERRolloutStorage)
+            self._rollouts = create_rollouts_fn(device=self._device)
+            return
         cls = baseline_registry.get_storage(hb.rollout_storage_name) or RolloutStorage
         obs_space = get_rollout_obs_space(self._env_spec.observation_space, self._actor_critic, self._config)
         self._rollouts = cls(self._ppo_cfg.num_steps, self._num_envs, obs_space,

@@ -67,6 +67,22 @@ int hb200_gae_adv(const float* rewards, float* value_preds, const uint8_t* masks
                   int t_cur, int t_alloc, int n_envs, float gamma, float tau, int use_gae,
                   int variant, hb200_stream_t stream);
 
+/* ---- VER: GAE over packed sequences ------------------------------------------------------
+ * replaces VERRolloutStorage.compute_returns (HB/rl/ver/ver_rollout_storage.py:430-568) fused with the advantages of
+ * PPO.get_advantages.  rewards, value_preds, returns (in/out), advantages: f32 [n_frames]; is_stale: u8 [n_frames].
+ * seq_table (int32, one upload per update): select_inds [n_frames] | step_offset [max_len] | seq_len [n_seqs] |
+ * last_for_env [n_seqs]: step t of sequence s (longest first) is frame
+ * select_inds[step_offset[t] + s]; last_for_env marks each environment's last sequence, whose last step is the
+ * bootstrap step (its return becomes NaN, its value bootstraps the step before).  A stale step keeps a finite old
+ * return.  use_gae = 0 means tau = 1.  gamma and tau are doubles, like the python floats the reference computes
+ * with; accumulation is fp64 in the reference's operation order.
+ * stats (f64[4]): sum, sum of squares and count of the finite advantages, count of finite returns.
+ * expected_finite >= 0: synchronise the stream and fail unless the finite-return count equals it.
+ */
+int hb200_ver_gae(const float* rewards, const float* value_preds, float* returns, const uint8_t* is_stale,
+                  const int32_t* seq_table, int n_frames, int n_seqs, int max_len, double gamma, double tau, int use_gae,
+                  float* advantages, double* stats, int expected_finite, hb200_stream_t stream);
+
 /* advantages <- (advantages - mean) * rsqrt(var + 1e-5) in place (ppo.py:151-153).
  * mode 0: single process, unbiased torch.var_mean over finite entries computed from stats
  * (ppo.py:155-157).  mode 1: mean/var given in mean_var[2] on device (distributed path,
@@ -497,6 +513,10 @@ int hb200_relu_bwd(float* d, const float* y, long long ld_d, long long ld_y, lon
  * the minibatch's cached visual features of a frozen encoder, read from the rollout storage for the visual_fc GEMM */
 int hb200_gather_rows(const float* src, const int32_t* frame_rows, float* out, int batch, long long row_elems,
                       hb200_stream_t stream);
+/* out[r, :cols] = idx[r] >= 0 ? src[idx[r], :cols] : 0 (f32, row pitches ld_src / ld_out): a VER minibatch's frames to
+ * and from the recurrence's zero-padded time-major [T_max, S] layout */
+int hb200_gather_rows_pad(const float* src, long long ld_src, const int32_t* idx, float* out, long long ld_out,
+                          int rows, int cols, hb200_stream_t stream);
 /* f32 [B, C*hw] flattened in (c,h,w) order (nn.Flatten of NCHW, resnet_policy.py:587-594)
  * -> bf16 NHWC [B,hw,C]: the gradient of visual_fc's input re-enters the NHWC conv stack */
 int hb200_f32_chw_to_bf16_hwc(const float* x, hb200_bf16* out, int batch, int hw, int channels,

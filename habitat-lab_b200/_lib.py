@@ -108,6 +108,7 @@ SIGNATURES = {
     "hb200_prev_action_linear_bwd": ("i", "ppii" + "p" + "ii" + "pp" + "p"),
     "hb200_prep_generic": ("i", "pppp" + "i" + "p" + "iii" + "pppp" + "p"),
     "hb200_obs_resample": ("i", "ppp" + "ii" + "p"),
+    "hb200_obs_project": ("i", "pppppp" + "ii" + "p"),
 }
 
 

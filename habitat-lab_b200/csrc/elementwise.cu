@@ -1241,11 +1241,12 @@ __global__ void prev_action_linear_bwd_kernel(const float* __restrict__ pa, cons
 // (ResNetEncoder.forward, resnet_policy.py:255-271: per-key permute, u8 keys scaled by 1 / high, channel concat,
 // avg_pool2d(2) -- the odd last row / column is dropped -- then RunningMeanAndVar.)  One thread per pooled pixel;
 // the fast rgb-u8 + depth-f32 kernels above stay the path for the PointNav sensor set.
+constexpr int kPrepMaxSrcs = 8;   // one channel each at most: the stem takes 8 input channels
 struct PrepSrcs {
-  const void* ptr[4];
-  int dtype[4];     // 0 u8, 1 f32, 2 i32
-  int channels[4];
-  float scale[4];   // multiplied BEFORE pooling (u8: 1 / high)
+  const void* ptr[kPrepMaxSrcs];
+  int dtype[kPrepMaxSrcs];     // 0 u8, 1 f32, 2 i32
+  int channels[kPrepMaxSrcs];
+  float scale[kPrepMaxSrcs];   // multiplied BEFORE pooling (u8: 1 / high)
   int n;
 };
 __device__ __forceinline__ float prep_load(const void* p, int dtype, size_t i) {
@@ -2359,12 +2360,15 @@ extern "C" int hb200_prep_generic(const void* const* h_srcs, const int* h_dtypes
                                   const float* h_scales, int n_srcs, const int32_t* frame_rows, int batch, int height,
                                   int width, const float* scale_shift, hb200_f16* out, hb200_bf16* out_bf16,
                                   double* stats_acc, hb200_stream_t stream) {
-  HB_CHECK_ARG(h_srcs && h_dtypes && h_channels && h_scales && n_srcs >= 1 && n_srcs <= 4, "prep_generic: 1..4 sources");
+  HB_CHECK_ARG(h_srcs && h_dtypes && h_channels && h_scales && n_srcs >= 1 && n_srcs <= kPrepMaxSrcs,
+               "prep_generic: 1..%d sources", kPrepMaxSrcs);
   HB_CHECK_ARG(frame_rows && batch > 0 && height >= 2 && width >= 2, "prep_generic: bad shape");
   HB_CHECK_ARG((stats_acc != nullptr) != (out != nullptr), "prep_generic: pass either stats_acc (statistics pass) or out (apply pass)");
   PrepSrcs src;
   int ctot = 0;
-  for (int k = 0; k < 4; ++k) { src.ptr[k] = nullptr; src.dtype[k] = 0; src.channels[k] = 0; src.scale[k] = 1.f; }
+  for (int k = 0; k < kPrepMaxSrcs; ++k) {
+    src.ptr[k] = nullptr; src.dtype[k] = 0; src.channels[k] = 0; src.scale[k] = 1.f;
+  }
   for (int k = 0; k < n_srcs; ++k) {
     HB_CHECK_ARG(h_srcs[k] && h_dtypes[k] >= 0 && h_dtypes[k] <= 2 && h_channels[k] >= 1, "prep_generic: bad source %d", k);
     src.ptr[k] = h_srcs[k]; src.dtype[k] = h_dtypes[k]; src.channels[k] = h_channels[k]; src.scale[k] = h_scales[k];

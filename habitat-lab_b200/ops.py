@@ -639,6 +639,69 @@ def obs_resample(keys):
     call("hb200_obs_resample", ctypes.addressof(src_a), ctypes.addressof(dst_a), ctypes.addressof(desc_a), n, batch)
 
 
+OBS_PROJECT_MAX_TARGETS = 8
+_PROJECT_MAX_FACES = 6
+
+
+def obs_project(jobs):
+    """Stitch NHWC image batches through projection tables, every target in one launch (CubeMap2Equirect,
+    CubeMap2Fisheye, Equirect2CubeMap).
+
+    jobs: list of (faces, dst, table, in_zf, out_zf): faces a list of n_in (1..6) [B, Hi, Wi, C] tensors of one
+    dtype (uint8, float32 or int32), Hi, Wi >= 3; table float32 [n_out, h, w, 3] (x, y, input) per output pixel
+    (common/projection.Stitch.table); dst [B * n_out, h, w, C] of the faces' dtype; in_zf None or float32 [n_in, Hi, Wi]
+    (input depth factors); out_zf None or float32 [n_out, h, w].  dst receives, bit for bit, what torch on the CPU
+    computes as grid_sample(face.float() * in_zf, grid, align_corners=True) summed over the faces, times out_zf,
+    .to(dtype).  Every tensor must be a contiguous CUDA tensor on one device; dst may be a view into a larger buffer."""
+    if not 1 <= len(jobs) <= OBS_PROJECT_MAX_TARGETS:
+        raise _lib.Hb200Error(f"obs_project: {len(jobs)} targets (1..{OBS_PROJECT_MAX_TARGETS} per launch)")
+    srcs, dsts, tabs, izs, ozs, desc, batch = [], [], [], [], [], [], None
+    for i, (faces, dst, table, in_zf, out_zf) in enumerate(jobs):
+        what = f"obs_project target {i}"
+        faces = list(faces)
+        if not 1 <= len(faces) <= _PROJECT_MAX_FACES:
+            raise _lib.Hb200Error(f"{what}: {len(faces)} input faces (1..{_PROJECT_MAX_FACES})")
+        f0 = faces[0]
+        if f0.dtype not in _PREP_DTYPE:
+            raise _lib.Hb200Error(f"{what}: dtype {f0.dtype} (uint8, float32 or int32)")
+        if f0.dim() != 4 or dst.dim() != 4 or table.dim() != 4 or table.shape[-1] != 3:
+            raise _lib.Hb200Error(f"{what}: expected NHWC faces / output and an [n_out, h, w, 3] table, got "
+                                  f"{tuple(f0.shape)} -> {tuple(dst.shape)} via {tuple(table.shape)}")
+        B, Hi, Wi, C = f0.shape
+        n_out, h, w, _ = table.shape
+        batch = B if batch is None else batch
+        for j, f in enumerate(faces):
+            _chk(f, f0.dtype, f"{what} face {j}")
+            if tuple(f.shape) != tuple(f0.shape) or f.device != f0.device:
+                raise _lib.Hb200Error(f"{what}: face {j} {tuple(f.shape)} on {f.device}, face 0 {tuple(f0.shape)} on "
+                                      f"{f0.device}")
+        _chk(dst, f0.dtype, f"{what} dst")
+        _chk(table, torch.float32, f"{what} table")
+        if B != batch or B == 0 or tuple(dst.shape) != (B * n_out, h, w, C):
+            raise _lib.Hb200Error(f"{what}: output {tuple(dst.shape)}, expected {(B * n_out, h, w, C)} (batch {batch})")
+        if Hi < 3 or Wi < 3:
+            raise _lib.Hb200Error(f"{what}: input faces of {Hi}x{Wi}: sampling needs at least 3x3")
+        if not 1 <= n_out <= _PROJECT_MAX_FACES or h == 0 or w == 0 or C == 0:
+            raise _lib.Hb200Error(f"{what}: table {tuple(table.shape)}, {C} channels")
+        for name, zf, want in (("in_zf", in_zf, (len(faces), Hi, Wi)), ("out_zf", out_zf, (n_out, h, w))):
+            if zf is not None:
+                _chk(zf, torch.float32, f"{what} {name}")
+                if tuple(zf.shape) != want:
+                    raise _lib.Hb200Error(f"{what}: {name} {tuple(zf.shape)}, expected {want}")
+        if any(t is not None and t.device != f0.device for t in (dst, table, in_zf, out_zf)):
+            raise _lib.Hb200Error(f"{what}: tensors on more than one device")
+        srcs += [f.data_ptr() for f in faces] + [None] * (_PROJECT_MAX_FACES - len(faces))
+        dsts.append(dst.data_ptr())
+        tabs.append(table.data_ptr())
+        izs.append(ptr(in_zf))
+        ozs.append(ptr(out_zf))
+        desc += [_PREP_DTYPE[f0.dtype], len(faces), n_out, Hi, Wi, C, h, w]
+    n = len(jobs)
+    arrs = [(ctypes.c_void_p * len(a))(*a) for a in (srcs, dsts, tabs, izs, ozs)]
+    desc_a = (ctypes.c_int32 * len(desc))(*desc)
+    call("hb200_obs_project", *[ctypes.addressof(a) for a in arrs], ctypes.addressof(desc_a), n, batch)
+
+
 # ---- experimental probes (not on the product path) ------------------------------------------------------
 def tma_halo_probe(x, out, b, oh0, ow0, halo_h, halo_w, pad):
     """x bf16 [B,H,W,C] -> out bf16 [C/8, halo_h, halo_w, 8]: one tile's input halo loaded by TMA (see hb200.h)."""

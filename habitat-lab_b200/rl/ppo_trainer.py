@@ -24,7 +24,7 @@ from ..common.baseline_registry import baseline_registry
 from ..common.obs_transformers import ObsTransformPlan, apply_obs_transforms_obs_space, get_active_obs_transforms
 from ..common.rollout_storage import RolloutStorage
 from ..common.tensor_dict import TensorDict
-from ..synthetic import pointnav_spaces
+from ..synthetic import cubemap_spaces, fill_image_, pointnav_spaces
 import os
 
 from .ppo import DDPPO, PPO  # noqa: F401  (registers the updaters)
@@ -83,7 +83,7 @@ class VERConfig:
 
 def make_config(num_environments=4, total_num_steps=-1.0, num_updates=2, height=256, width=256, seed=100,
                 obs_transforms=None, ddppo=None, continuous_actions=0, action_dist=None, trainer_name="ddppo",
-                ver=None, step_time_spread=0.0, **ppo_kw):
+                ver=None, step_time_spread=0.0, cubemap=None, **ppo_kw):
     """A habitat_baselines-shaped config for the synthetic PointNav DD-PPO run (ddppo_pointnav.yaml values).
     obs_transforms: {name: config node with `type` and the transformer's fields} (e.g. the ObjectNav YAMLs'
     resize_shortest_edge + center_cropper, common/obs_transformers.py); height / width are then the raw sensor size.
@@ -93,7 +93,9 @@ def make_config(num_environments=4, total_num_steps=-1.0, num_updates=2, height=
     dict(use_std_param=True)).
     trainer_name="ver": Variable Experience Rollout (rl/ver_trainer.py) with `ver` the VERConfig field overrides;
     step_time_spread > 0 gives every synthetic environment step its own duration on a seeded virtual clock, so
-    environments contribute unequal numbers of steps to a rollout."""
+    environments contribute unequal numbers of steps to a rollout.
+    cubemap="rgb" / "depth": the synthetic environment is a cube-map rig (synthetic.cubemap_spaces) of six height x
+    height faces `{cubemap}_0` .. `{cubemap}_5`, for CubeMap2Equirect / CubeMap2Fisheye."""
     ppo = PPOConfig(**{**dict(ppo_epoch=2, num_mini_batch=2, num_steps=128, max_grad_norm=0.2), **ppo_kw})
     agent = SimpleNamespace(name="PointNavResNetPolicy", action_distribution_type="categorical")
     if continuous_actions:
@@ -113,8 +115,13 @@ def make_config(num_environments=4, total_num_steps=-1.0, num_updates=2, height=
     habitat = SimpleNamespace(seed=seed, simulator=SimpleNamespace(agents_order=["main_agent"]),
                               synthetic=SimpleNamespace(height=height, width=width, p_done=1.0 / 250.0,
                                                         continuous_actions=int(continuous_actions),
-                                                        step_time_spread=float(step_time_spread)))
+                                                        step_time_spread=float(step_time_spread),
+                                                        cubemap=cubemap))
     return SimpleNamespace(habitat_baselines=hb, habitat=habitat)
+
+
+# torch dtype of each image dtype a synthetic camera can have
+_IMAGE_DTYPE = {np.dtype(np.uint8): torch.uint8, np.dtype(np.float32): torch.float32, np.dtype(np.int32): torch.int32}
 
 
 # ---- synthetic VectorEnv ------------------------------------------------------------------------------
@@ -149,6 +156,10 @@ class SyntheticVectorEnv:
             out["rgb"] = torch.randint(0, 256, (n, *sp["rgb"].shape), generator=g, device=d, dtype=torch.uint8)
         if "depth" in sp:
             out["depth"] = torch.rand((n, *sp["depth"].shape), generator=g, device=d)
+        for k, s in sp.items():   # any other camera (the cube-map rig's faces), filled by dtype
+            if k not in ("rgb", "depth") and len(s.shape) == 3:
+                out[k] = torch.empty((n, *s.shape), dtype=_IMAGE_DTYPE[np.dtype(s.dtype)], device=d)
+                fill_image_(out[k], g, d)
         goal = torch.rand(n, 2, generator=g, device=d)
         goal[:, 0] *= 10.0
         goal[:, 1] = goal[:, 1] * 2 * math.pi - math.pi
@@ -199,7 +210,10 @@ class SyntheticVectorEnvFactory:
     def construct_envs(self, config, workers_ignore_signals=False, enforce_scenes_greater_eq_environments=False,
                        is_first_rank=True, device=None, rank=0):
         syn = config.habitat.synthetic
-        obs_space, act_space = pointnav_spaces(syn.height, syn.width)
+        if getattr(syn, "cubemap", None):
+            obs_space, act_space = cubemap_spaces(syn.height, syn.cubemap)
+        else:
+            obs_space, act_space = pointnav_spaces(syn.height, syn.width)
         if getattr(syn, "continuous_actions", 0):   # the environment draws no random numbers for its actions
             act_space = spaces.Box(-1.0, 1.0, (syn.continuous_actions,), np.float32)
         n = config.habitat_baselines.num_environments

@@ -45,6 +45,29 @@ def imagenav_spaces(H=256, W=256, n_actions=4):
     return spaces.Dict(od), spaces.Discrete(n_actions)
 
 
+def cubemap_spaces(face=256, sensor="depth", n_actions=4):
+    """A cube-map rig for CubeMap2Equirect / CubeMap2Fisheye: six face x face cameras `{sensor}_0` .. `{sensor}_5` in
+    the order Back, Down, Front, Left, Right, Up ("rgb": u8 x3, "depth": f32 x1 in [0, 1]), plus the point goal."""
+    if sensor not in ("rgb", "depth"):
+        raise ValueError(f"cubemap_spaces: sensor {sensor!r} (rgb or depth)")
+    box = spaces.Box(0, 255, (face, face, 3), np.uint8) if sensor == "rgb" else \
+        spaces.Box(0.0, 1.0, (face, face, 1), np.float32)
+    od = {f"{sensor}_{i}": box for i in range(6)}
+    od["pointgoal_with_gps_compass"] = spaces.Box(np.finfo(np.float32).min, np.finfo(np.float32).max, (2,),
+                                                  np.float32)
+    return spaces.Dict(od), spaces.Discrete(n_actions)
+
+
+def fill_image_(t, g, dev):
+    """Synthetic image values by dtype: u8 uniform, int32 class ids 0..39, f32 uniform [0, 1)."""
+    if t.dtype == torch.uint8:
+        t.copy_(torch.randint(0, 256, t.shape, generator=g, device=dev, dtype=torch.uint8))
+    elif t.dtype == torch.int32:
+        t.copy_(torch.randint(0, 40, t.shape, generator=g, device=dev, dtype=torch.int32))
+    else:
+        t.copy_(torch.rand(t.shape, generator=g, device=dev))
+
+
 def fill_observations_(obs, observation_space, g, dev, chunk_steps: int = 8):
     """Synthetic values for ANY sensor of `observation_space` by dtype / rank: images chunk by chunk (u8 uniform, f32
     uniform [0,1), int32 class ids 0..39), 1-D sensors by name (angles uniform in [-pi, pi), categories uniform over the
@@ -54,13 +77,7 @@ def fill_observations_(obs, observation_space, g, dev, chunk_steps: int = 8):
         T1 = t.shape[0]
         if len(sp.shape) == 3:
             for t0 in range(0, T1, chunk_steps):
-                t1 = min(T1, t0 + chunk_steps)
-                if t.dtype == torch.uint8:
-                    t[t0:t1] = torch.randint(0, 256, t[t0:t1].shape, generator=g, device=dev, dtype=torch.uint8)
-                elif t.dtype == torch.int32:
-                    t[t0:t1] = torch.randint(0, 40, t[t0:t1].shape, generator=g, device=dev, dtype=torch.int32)
-                else:
-                    t[t0:t1] = torch.rand(t[t0:t1].shape, generator=g, device=dev)
+                fill_image_(t[t0:min(T1, t0 + chunk_steps)], g, dev)
         elif t.dtype == torch.int64:
             t.copy_(torch.randint(0, int(sp.high.max()) + 1, t.shape, generator=g, device=dev))
         elif k == "pointgoal_with_gps_compass":

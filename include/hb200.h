@@ -582,7 +582,7 @@ int hb200_prev_action_linear_fwd(const float* prev_actions, const uint8_t* masks
 int hb200_prev_action_linear_bwd(const float* prev_actions, const uint8_t* masks, int batch, int n_actions,
                                  const float* d_out, int ld, int col0, float* d_w, float* d_b, hb200_stream_t stream);
 /* Generic visual input prep (ResNetEncoder.forward, HB/rl/ddppo/policy/resnet_policy.py:255-271) for ANY sensor mix
- * and size: up to 4 HWC sources (h_* are HOST arrays of n_srcs entries: device pointers, dtype 0 u8 / 1 f32 / 2 i32,
+ * and size: up to 8 HWC sources (h_* are HOST arrays of n_srcs entries: device pointers, dtype 0 u8 / 1 f32 / 2 i32,
  * channels, pre-pool scale = 1/high for u8 keys), <= 8 channels in total, concatenated in order, avg_pool2d(2) (odd
  * last row / column dropped).  stats_acc != NULL: statistics pass (17 doubles like hb200_prep_stats); otherwise the
  * apply pass writes out f16 [batch, H/2, W/2, 8] (+ optional bf16 twin) normalised with scale_shift (NULL: raw). */
@@ -600,6 +600,20 @@ int hb200_prep_generic(const void* const* h_srcs, const int* h_dtypes, const int
  * (Hr = H, Wr = W: the window's bits).  Pointers must be aligned to their element size; src and dst must not overlap. */
 int hb200_obs_resample(const void* const* src, void* const* dst, const int32_t* desc, int n_keys, int batch,
                        hb200_stream_t stream);
+
+/* Cube-map projection transforms (HB/common/obs_transformers.py CubeMap2Equirect, CubeMap2Fisheye, Equirect2CubeMap)
+ * for NHWC batches, every target in ONE launch.  All arguments but the stream are HOST arrays over n_targets (<= 8):
+ * src[6 * i + j]: input face j of target i, [batch, Hi, Wi, C] (entries past n_in unused); dst[i]: a contiguous
+ * [batch, n_out, h, w, C] region; table[i]: [n_out, h, w, 3] float (x, y, input) per output pixel, the normalised
+ * align_corners sampling point in the assigned input (input -1: the pixel is 0); in_zf[i]: NULL or [n_in, Hi, Wi]
+ * depth factors applied to input pixels before sampling; out_zf[i]: NULL or [n_out, h, w] factors applied after.
+ * desc: 8 ints per target: dtype (0 u8, 1 f32, 2 i32), n_in (1..6), n_out (1..6), Hi, Wi (>= 3), C, h, w.  Each output
+ * is bit-identical to torch on the CPU summing grid_sample(img.float() * in_zf, grid, align_corners=True) over the
+ * inputs, times out_zf, .to(dtype).  Pointers must be aligned to their element size; inputs and outputs must not
+ * overlap. */
+int hb200_obs_project(const void* const* src, void* const* dst, const float* const* table, const float* const* in_zf,
+                      const float* const* out_zf, const int32_t* desc, int n_targets, int batch,
+                      hb200_stream_t stream);
 
 /* Not on the product path yet: mechanism probe (verified on hardware) for the TMA halo load of the halo convolutions
  * (NOTES_NEXT.md): loads the halo_h x halo_w halo of the tile whose first output pixel is (oh0, ow0) of frame b from the
